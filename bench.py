@@ -16,8 +16,10 @@ oracle's run of the same workload (made once, outside the timed regions, on host
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
            --master-port 29500 bench.py --gpus 8 --steps 5 --warmup 3
     python bench.py --impl reference          # the CPU oracle (port of the reference path) on the host cores
+    python bench.py --dump-outputs DIR        # also write what the last timed step computed, as DIR/*.npy
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -32,7 +34,8 @@ sys.path.insert(0, ROOT)
 
 METRIC = "gossip edge-updates/sec @10M nodes"
 UNIT = "edge-updates/s"
-HBM_FALLBACK_GBS = 6650.0          # B200_PROFILING.md fallback when MEASURED_PEAKS.json is absent
+HBM_FALLBACK_GBS = 3350.0          # H100 SXM data sheet (HBM3), used when MEASURED_PEAKS.json is absent
+DUMP_BYTES = 64_000_000           # --dump-outputs: at most this many bytes in all
 
 
 def make_scenario(args, nodes=None):
@@ -53,17 +56,17 @@ def config_dict(args, name, slots):
             if args.workload == "leave_fail" else f"{slots} tracked subject(s) leave at tick 0")
     return {"workload": f"configs[3] shape: {args.nodes}-node random graph (out-degree {args.degree}), fanout={args.fanout}, {what}, run to quiescence",
             "scenario": name, "nodes": args.nodes, "degree": args.degree, "fanout": args.fanout, "slots": slots,
-            "retransmit_mult": 4, "cache": "member records (%d MB) + CSR (%d MB) exceed the 126 MB L2; no flush needed"
+            "retransmit_mult": 4, "cache": "member records (%d MB) + CSR (%d MB) exceed the 50 MB L2; no flush needed"
             % (args.nodes * 32 * slots // 2**20, args.nodes * args.degree * 4 // 2**20)}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons (B200_PROFILING.md recipe).  nvidia-smi needs ~1 s to start, so it is
+    """nvidia-smi clocks / throttle reasons / power limit.  nvidia-smi needs ~1 s to start, so it is
     launched before the warm-up; samples are time-stamped and only those inside [mark_begin, mark_end] — the timed
     regions — are summarised (all samples under load if the window caught none)."""
 
     QUERY = "timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-            "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+            "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name"
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -74,6 +77,7 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), f"--query-gpu={self.QUERY}", "--format=csv,noheader,nounits", "-lms", "20"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             threading.Thread(target=self._pump, daemon=True).start()
+            atexit.register(self.proc.terminate)        # never outlive the benchmark, also when a self-check exits early
         except OSError:
             self.proc = None
 
@@ -92,9 +96,10 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.1)
         self.proc.terminate()
+        self.proc.wait()
 
         def summarise(rows):
-            sm, mx, reasons = [], [], set()
+            sm, mx, reasons, card = [], [], set(), {}
             for _, r in rows:
                 try:
                     sm.append(float(r[1])); mx.append(float(r[2]))
@@ -103,14 +108,16 @@ class ClockSampler:
                 for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[4:8]):
                     if v.lower().startswith("active"):
                         reasons.add(name)
-            return sm, mx, reasons
+                if len(r) > 9:
+                    card = {"gpu": r[9], "power_limit_w": r[8]}
+            return sm, mx, reasons, card
         inside = [x for x in self.rows if self.t0 is not None and self.t0 <= x[0] <= (self.t1 or 1e30)]
         window = "timed regions"
         if not inside:
             inside, window = self.rows, "warm-up + timed regions (no sample fell inside the timed window)"
-        sm, mx, reasons = summarise(inside)
+        sm, mx, reasons, card = summarise(inside)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "samples": len(sm), "window": window, "reasons": sorted(reasons)}
+                "samples": len(sm), "window": window, "reasons": sorted(reasons), **card}
 
 
 def b_edge(fanout, p_dirty):
@@ -215,6 +222,27 @@ def run_reference(args):
     print(json.dumps(line))
 
 
+def dump_outputs(g, sc, ticks, ok, out_dir, rank, world):
+    """What a caller of the timed path receives from its last step: the run's outcome and totals, and per node the member
+    status and status Lamport time of every tracked subject and the node's Lamport clock.  Per-node vectors are a fixed,
+    seeded sample of the shard's nodes (all of them when they fit) so that the files stay under DUMP_BYTES in all; every
+    value is exact in the float type it is stored as.  Sharded runs write one set per rank, prefixed rank<r>_."""
+    st, h = g.stats(), int(g.state_hash())             # collective when sharded: every rank calls both
+    per_node = 8 + 8 + sc.slots * (4 + 8)              # node id and clock (float64), status (float32) + status time (float64) per slot
+    k = min(g.count, (DUMP_BYTES - 4096) // world // per_node)
+    local = np.arange(g.count) if k == g.count else np.sort(np.random.default_rng(20240901 + rank).choice(g.count, k, replace=False))
+    pre = f"rank{rank}_" if world > 1 else ""
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"run": np.array([ticks, ok, st["edge_updates"], st["messages"], st["changed"], st["packets"], h >> 32, h & 0xFFFFFFFF], dtype=np.float64),
+           "node_id": (local + g.first).astype(np.float64),
+           "lamport_time": g.lamport_time()[local].astype(np.float64)}
+    for s in range(sc.slots):
+        out[f"member_status_slot{s}"] = g.member_status(s)[local].astype(np.float32)
+        out[f"status_ltime_slot{s}"] = g.status_ltime(s)[local].astype(np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, pre + name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -232,6 +260,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-numa-bind", action="store_true", help="A/B: leave the driver thread where the OS scheduler puts it")
     ap.add_argument("--no-check", action="store_true", help="skip the full-size oracle run every step is checked against")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last one computed as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -346,13 +375,15 @@ def main():
     t0 = time.perf_counter()
     d2h = 0
     for k in range(args.steps):
-        _, _, _, _, ob = one_step(pins[k & 1])
-        d2h = ob
+        last = one_step(pins[k & 1])
+        d2h = last[4]
     g.results_wait()                                     # the last copies have landed in host memory
     sync_all()
     wall_e2e = time.perf_counter() - t0
     sampler.mark_end()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:                                # outside the sampled window; the state is that of the last timed step
+        dump_outputs(g, sc, last[0], last[1], args.dump_outputs, rank, world)
     if expect is not None:                               # the vectors that came back are the converged ones: every other node sees the leaver as Left
         from serf_b200 import MemberStatus
         stv = pins[(args.steps - 1) & 1]["status"][0].numpy()
@@ -376,16 +407,9 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         else:
-            peak, peak_src = HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+            peak, peak_src = HBM_FALLBACK_GBS, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
         tick_launches = launches                       # kernels of the executed ticks (tick kernels ≥ 98 % of them; launches past the quiescent tick return at once and are not counted)
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", f"r2_traffic_{args.workload}.json")      # ncu capture of THIS workload with the shipped kernel
-        if world == 1 and os.path.exists(tpath):
-            tj = json.load(open(tpath))
-            # DRAM bytes of ONE run of this workload (every tick_kernel launch of the capture) over the launches of one bench step: the same
-            # denominator as algorithmic_bytes_per_launch (launches that return at once — gated ticks, the idle half of a dual launch — count in both)
-            traffic = (tj.get("dram_bytes_read", 0.0) + tj.get("dram_bytes_write", 0.0)) / max(1.0, launches / args.steps)
-            traffic_src = f"{os.path.relpath(tpath, ROOT)} (ncu dram__bytes_read.sum + dram__bytes_write.sum over all tick_kernel launches of one run, per launch of a bench step; {tj.get('source', '')})"
+        traffic, traffic_src = None, "not measured (needs DRAM counters, which a CUDA-event timing does not give)"
         # per-GPU: each GPU runs its own tick kernel over its shard; algorithmic bytes split evenly
         achieved = (total_eu / world) * be / (dev_ms * 1e-3) / 1e9
         h2d = len(sc.ops) * 12

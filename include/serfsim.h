@@ -1,5 +1,5 @@
 /*
- * serfsim.h — C ABI of the B200 gossip-dissemination simulator (drop-in boundary).
+ * serfsim.h — C ABI of the H100 gossip-dissemination simulator (drop-in boundary).
  *
  * This is the seam a serf-core `Transport`/`Delegate` shim binds to (Rust `extern "C"` /
  * cudarc-style FFI, see INTEGRATION.md).  Every entry point names the reference
@@ -18,7 +18,7 @@
  *   - Lamport times are u64 at this boundary (`types/clock.rs:14`); the device keeps
  *     them as u32 and every call fails with SERFSIM_E_OVERFLOW instead of wrapping.
  *
- * The only backend is CUDA (sm_100a).  There is no CPU fallback: serfsim_create fails
+ * The only backend is CUDA (sm_90a).  There is no CPU fallback: serfsim_create fails
  * with SERFSIM_E_NO_DEVICE when no usable GPU is present.
  */
 #ifndef SERFSIM_H

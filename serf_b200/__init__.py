@@ -1,6 +1,6 @@
-"""serf_b200 — B200-native simulator of serf's SWIM gossip dissemination hot path.
+"""serf_b200 — H100-native simulator of serf's SWIM gossip dissemination hot path.
 
-The product is `libserfsim.so` (hand-written sm_100a CUDA kernels behind the C ABI of
+The product is `libserfsim.so` (hand-written sm_90a CUDA kernels behind the C ABI of
 include/serfsim.h).  This package is the thin ctypes driver used by the tests and the
 bench; it mirrors serf-core's names (MemberStatus, Serf::join/leave/…, Stats).
 """

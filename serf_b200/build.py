@@ -1,4 +1,4 @@
-"""Builds serf_b200/libserfsim.so (CUDA kernels + C ABI) in-tree for sm_100a with nvcc."""
+"""Builds serf_b200/libserfsim.so (CUDA kernels + C ABI) in-tree for sm_90a with nvcc."""
 import os
 import shutil
 import subprocess
@@ -29,7 +29,7 @@ def is_stale():
 def build(force=False, verbose=False):
     if not force and not is_stale():
         return OUT
-    cmd = [nvcc_path(), "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    cmd = [nvcc_path(), "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
            "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-shared", "-o", OUT]
     if verbose:
         cmd += ["-Xptxas", "-v"]

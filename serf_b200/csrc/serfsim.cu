@@ -664,10 +664,11 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(SERFSIM_E_NO_DEVICE, "no CUDA device: serfsim has no CPU execution path");
   if (cfg->device >= 0) { if (cfg->device >= ndev) return fail(SERFSIM_E_NO_DEVICE, "device ordinal out of range"); CU(cudaSetDevice(cfg->device)); }
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   CU(cudaGetDevice(&dev));
   CU(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 10) return fail(SERFSIM_E_NO_DEVICE, "kernels are built for sm_100a only (B200)");
+  CU(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  if (major != 9 || minor != 0) return fail(SERFSIM_E_NO_DEVICE, "kernels are built for sm_90a only (H100)");
 
   serfsim* h = new serfsim();
   h->cfg = *cfg; h->N = cfg->n_nodes; h->R = cfg->slots;
@@ -730,7 +731,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
     cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev);
     cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, dev);
     h->l2_persist_max = (size_t)max_persist; h->l2_window_max = (size_t)max_window;
-    int want = 0;        // measured: a 79 MB persisting carve-out makes the plateau tick 35 % slower (profiles/r1_notes.md)
+    int want = 0;        // off by default: a carve-out takes L2 away from the streamed planes and the inbox alike
     if (const char* e = getenv("SERFSIM_L2_PERSIST")) want = atoi(e);
     if (want && max_persist > 0) cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)max_persist);
     if (const char* e = getenv("SERFSIM_L2_WINDOW")) h->l2_window = atoi(e) != 0;
@@ -831,7 +832,7 @@ int serfsim_set_topology_csr(serfsim_t* h, const uint64_t* row_ptr, const uint32
   // TMA pipeline (single-slot runs): a stage holds the largest tile's CSR span if that is at most 48 KB
   h->stage_col_bytes = 0;
   {
-    int use = 0;   // measured (profiles/): the direct-load kernel is 3 % faster over a whole run; SERFSIM_TMA=1 selects the TMA pipeline
+    int use = 0;   // the direct-load kernel is the default (DESIGN §5); SERFSIM_TMA=1 selects the TMA pipeline
     if (const char* e = getenv("SERFSIM_TMA")) use = atoi(e);
     const u32 need = std::max<u32>(h->max_tile_edges * 4u, 16u);
     if (use && h->R == 1 && need <= 48u * 1024u) h->stage_col_bytes = (need + 127u) & ~127u;

@@ -1,4 +1,4 @@
-// tick_kernel.cu — the fused gossip tick for sm_100a.
+// tick_kernel.cu — the fused gossip tick for sm_90a.
 //
 // One launch = one gossip tick of every virtual node of this shard:
 //   Phase R  receive: fold the reduced inbox of the previous tick into the node's views
@@ -13,8 +13,8 @@
 // Sends of tick t land in inbox parity t&1 and are consumed by Phase R of tick t+1, so a launch
 // never reads what it writes: bulk-synchronous, order-independent, bit-reproducible.
 //
-// Memory behaviour (HBM-bound integer work, no tensor cores): one thread per node; a node's 32-byte record is one
-// 256-bit load (LDG.E.256 = one DRAM sector, a warp covers 1 KB contiguous) and, if changed, one 256-bit store; node
+// Memory behaviour (HBM-bound integer work, no tensor cores): one thread per node; a node's 32-byte record is one DRAM
+// sector, read as two back-to-back 128-bit loads (a warp covers 1 KB contiguous) and, if changed, written as two; node
 // word, busy byte, inbox words and row offsets are coalesced streams with an evict_first / no-L1-allocate policy; the
 // four neighbour gathers stay inside the node's own 64-byte CSR row; the sends are 32-bit RED.MAX to random peers with
 // an evict_last policy — the inbox planes are the only randomly addressed data and are sized to stay L2-resident.
@@ -32,14 +32,17 @@ namespace {
 
 constexpr int BLOCK = 256;
 #ifndef SFS_MB_R1
-#define SFS_MB_R1 4                         // resident CTAs per SM of the single-slot kernels (64 registers per thread)
+// Resident CTAs per SM, i.e. the register cap of each kernel.  Spilled registers go through the LSU the kernels are bound by,
+// so the caps are the fastest ones of a sweep on the H100 (DESIGN §5): at 4 CTAs / 64 registers the single-slot kernel
+// spills 120–316 B per thread on sm_90a, at 2 CTAs / 128 registers the multi-slot kernel 390–640 B.
+#define SFS_MB_R1 3                         // single-slot kernels (80 registers per thread)
 #endif
 #ifndef SFS_MB_R1S
-#define SFS_MB_R1S SFS_MB_R1                // … of the sharded single-slot kernel (its send path needs more registers: A/B in profiles/r2_notes.md)
+#define SFS_MB_R1S SFS_MB_R1                // … of the sharded single-slot kernel (its send path needs more registers)
 #endif
 #ifndef SFS_MB_RN
-#define SFS_MB_RN 2                         // resident CTAs per SM of the multi-slot kernels (128 registers per thread: at 3 CTAs / 80 registers the
-#endif                                      // view loop spills, and local-memory traffic goes through the LSU the kernel is bound by: −7 % per run, profiles/r2_notes.md)
+#define SFS_MB_RN 1                         // multi-slot kernels (up to 255 registers per thread; ptxas uses about 200)
+#endif
 constexpr u32 TILE_SHIFT = 8;              // one tile = one CTA pass = 256 nodes
 constexpr u32 MAX_TILES_PER_CTA = 1024;
 static_assert((1u << TILE_SHIFT) == BLOCK, "tile = block");
@@ -48,22 +51,26 @@ static_assert((1u << TILE_SHIFT) == BLOCK, "tile = block");
 // The only randomly addressed data of a tick are the inbox planes the sends reduce into (RED.MAX,
 // 4 B at a random node).  They are kept L2-resident with an evict_last policy; everything that is
 // streamed exactly once per tick (records, node state, the inbox parity being consumed) goes
-// through evict_first / no-L1-allocate so it does not push the inbox out of the 126 MB L2.
+// through evict_first / no-L1-allocate so it does not push the inbox out of the 50 MB L2.
 struct Words { u32 w[8]; };   // one 32-byte record
 
 #ifndef SERFSIM_EMU
 __device__ __forceinline__ u64 policy_evict_first() { u64 p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p; }
 __device__ __forceinline__ u64 policy_evict_last() { u64 p; asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p; }
 
-__device__ __forceinline__ Words ld_rec256(const uint4* ptr, u64 pol) {   // one 256-bit load = one DRAM sector
+// sm_90 has no 256-bit LDG/STG: a record is two 128-bit accesses to the two halves of the same 32-byte sector, issued
+// back to back so that both are in flight together (the sector crosses DRAM once; the second half is served by L2).
+__device__ __forceinline__ Words ld_rec256(const uint4* ptr, u64 pol) {
   Words r;
-  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8], %9;"
+  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%8], %9;\n\t"
+               "ld.global.L1::no_allocate.L2::cache_hint.v4.u32 {%4,%5,%6,%7}, [%8+16], %9;"
                : "=r"(r.w[0]), "=r"(r.w[1]), "=r"(r.w[2]), "=r"(r.w[3]), "=r"(r.w[4]), "=r"(r.w[5]), "=r"(r.w[6]), "=r"(r.w[7])
                : "l"(ptr), "l"(pol));
   return r;
 }
 __device__ __forceinline__ void st_rec256(uint4* ptr, const Words& r, u64 pol) {
-  asm volatile("st.global.L2::cache_hint.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8}, %9;"
+  asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %9;\n\t"
+               "st.global.L2::cache_hint.v4.u32 [%0+16], {%5,%6,%7,%8}, %9;"
                :: "l"(ptr), "r"(r.w[0]), "r"(r.w[1]), "r"(r.w[2]), "r"(r.w[3]), "r"(r.w[4]), "r"(r.w[5]), "r"(r.w[6]), "r"(r.w[7]), "l"(pol) : "memory");
 }
 __device__ __forceinline__ u64 ld_u64_stream(const u64* ptr, u64 pol) {
@@ -138,7 +145,7 @@ struct StageView {
 
 struct Counters {          // per-thread, reduced once per CTA; rare counters (events, suspects) go straight to the trace row
   u32 packets, edges, changed, pending, kL, kJ, kM, views;
-  // single-view kernels (64 registers per thread, on the edge of spilling) keep six of them in three: a thread visits at most
+  // single-view kernels (tight register cap) keep six of them in three: a thread visits at most
   // MAX_TILES_PER_CTA = 1024 nodes, each adds at most MAX_FANOUT = 8 to a counter — 16 bits hold that
   u32 pe /* packets | edges << 16 */, cp /* changed | pending << 16 */, kLJ /* kL | kJ << 16 */;
   u64 hash;
@@ -215,9 +222,8 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
 // contiguous bytes over NVLink).  Space in a peer's window is reserved with an atomic on this rank's per-peer counter — one
 // flush AHEAD: after its blocks have been written, the lane whose index is the peer's rank reserves as many entries as this
 // flush used and keeps base and length in its own registers (`resv`, `rlen`); nothing reads them before the next flush, so the
-// atomic's round trip on a counter the whole grid hammers is off the critical path (reserving at flush time cost 17 % of the
-// sharded kernel's stall samples, profiles/r2g_hot_loop8_tick13.txt; so did a reservation issued inside the per-peer loop,
-// whose next warp shuffle had to wait for it, profiles/r2h_hot_loop8_tick13.txt).  In saturated ticks the first reservation is
+// atomic's round trip on a counter the whole grid hammers is off the critical path (a reservation at flush time, or one issued
+// inside the per-peer loop, puts that round trip in front of the next warp shuffle).  In saturated ticks the first reservation is
 // made when the kernel starts.  A flush that needs more than it holds takes the rest synchronously.  Reserved entries that stay
 // unwritten read as zeros at the receiver: the drain kernel skips zero entries and clears every entry it consumes, so a window
 // is all zeros again before it is written next.  force = false: whole blocks only; force = true (end of the kernel): everything.
@@ -351,7 +357,7 @@ __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool k
   const u32 nl = p.stride, R = p.R, s_hi = R1 ? 1u : R;
   Pre x;
   x.busy = p.busy[vl];
-  x.nd = (!R1 && due) ? p.node_due[vl] : NO_DEADLINE;    // single-view kernels (64 registers) read it where it is needed instead: one register less across the tile loop
+  x.nd = (!R1 && due) ? p.node_due[vl] : NO_DEADLINE;    // single-view kernels (tight register cap) read it where it is needed instead: one register less across the tile loop
   x.keep = R1 ? 0u : keep;
   x.mL = x.mJ = x.mM = x.qw = 0; x.any = 0; x.mailmask = 0; x.qmask = 0;
   for (u32 s2 = 0; s2 < s_hi; ++s2) {
@@ -377,8 +383,8 @@ __device__ __forceinline__ bool node_active(const TickParams& p, const Pre& x, b
 // Multi-slot runs, saturated ticks: what a node needs beyond its `Pre` words, requested ONE TILE AHEAD together with them — the node
 // word, the neighbour ids of its gossip peers (uniform out-degree: the row offset is arithmetic, the draw needs only tick and id) and the
 // record of the view it will most probably visit first (`keep`: the first view this thread visited in its previous tile; in a
-// dissemination wave nearly every node has the same views active).  The multi-slot kernel holds 16 warps per SM (128 registers per
-// thread): without this every tile pays three dependent round trips (Pre → node word + record → neighbour ids) with too few warps to
+// dissemination wave nearly every node has the same views active).  The multi-slot kernel holds 8 warps per SM (one CTA of 256 threads,
+// ≈ 200 registers per thread): without this every tile pays three dependent round trips (Pre → node word + record → neighbour ids) with too few warps to
 // hide them.  A guess that turns out wrong costs one unused 32-byte load; results never depend on it.
 template <int FMAX>
 struct Ahead { u64 ns; Words rec; u32 cand[FMAX]; u32 valid; };
@@ -1528,7 +1534,7 @@ int tick_grid_size(u32 n_local, int ctas_per_sm) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   const u32 tiles = (n_local + BLOCK - 1) / BLOCK;
   static int mul = 0;

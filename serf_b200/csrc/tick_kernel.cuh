@@ -12,7 +12,7 @@
 #endif
 #ifndef SERFSIM_EMU
 #define SFS_LAUNCH(grid, block, smem, stream, ...) __VA_ARGS__<<<(grid), (block), (smem), (stream)>>>
-constexpr int SFS_SMS = 148;                 // B200: grid-stride helper kernels are sized in multiples of the SM count
+constexpr int SFS_SMS = 132;                 // H100 SXM: grid-stride helper kernels are sized in multiples of the SM count
 #else
 constexpr int SFS_SMS = 1;
 #endif
@@ -134,8 +134,8 @@ constexpr u32 SCHED_TICKET = 0, SCHED_IDLE_UNTIL = 1, SCHED_UE_ACTIVITY = 2, SCH
               SCHED_VIEWS_NEW = 8 /* single-view ticks: bit s = view s can have business, in the ticks from SCHED_VIEWS_FROM on */, SCHED_VIEWS_NEXT = 9 /* being collected */,
               SCHED_VIEWS_OLD = 10 /* the set of the tick before SCHED_VIEWS_FROM */, SCHED_VIEWS_FROM = 11, SCHED_WORDS = 12;
 // Single-view ticks (multi-slot runs).  In long stretches of a study exactly one tracked subject is in motion (the suspicion and dead waves
-// of a crash after the leave wave has died down): every node visits the same single view, and the lean single-slot kernel (64 registers,
-// 32 warps per SM, every load requested up front) does that tick in half the time of the multi-slot kernel (128 registers, 16 warps).
+// of a crash after the leave wave has died down): every node visits the same single view, and the lean single-slot kernel (80 registers,
+// 24 warps per SM, every load requested up front) does that tick faster than the multi-slot kernel (one CTA of 8 warps per SM).
 // Which views can have business in tick t+1 is known at the end of tick t: views that sent mail or keep a queue (collected by the tick
 // kernel, the anti-entropy kernel and — across shards — the drain kernel in SCHED_VIEWS_*), plus what the host knows (views_host: every
 // subject that has ever been down — only those are probed, suspected and run timers; all views when the tick carries a host operation or a

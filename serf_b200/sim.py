@@ -166,7 +166,7 @@ def load_library():
     path = library_path()
     if not os.path.exists(path):
         raise SerfsimError(-2, f"{path} is missing: build it with `python -m serf_b200.build` "
-                               "(nvcc, sm_100a); there is no CPU fallback")
+                               "(nvcc, sm_90a); there is no CPU fallback")
     lib = C.CDLL(path)
     if hasattr(lib, "emu_probe"):             # tests/emu's host-compiled build of the kernels is test infrastructure, never the product
         raise SerfsimError(-2, f"{path} is the host-compiled test build (tests/emu), not the CUDA library: refusing to use it as the product")

@@ -1,6 +1,6 @@
 // Compiles the C++ host layer (include/serfsim.hpp) against libserfsim.so and checks, without a GPU, that the boundary
 // behaves as documented: the library loads, the ABI version matches, and creating a cluster fails loudly with
-// SERFSIM_E_NO_DEVICE (there is no CPU execution path).  On a B200 it runs the configs[0] scenario instead.
+// SERFSIM_E_NO_DEVICE (there is no CPU execution path).  On an H100 it runs the configs[0] scenario instead.
 #include <cstdio>
 #include <cstring>
 

@@ -122,7 +122,7 @@ typedef struct emuStream_st* cudaStream_t;
 typedef struct emuEvent_st* cudaEvent_t;
 enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3 };
 enum { cudaStreamNonBlocking = 1 };
-enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16, cudaDevAttrComputeCapabilityMajor = 75, cudaDevAttrMaxPersistingL2CacheSize = 108, cudaDevAttrMaxAccessPolicyWindowSize = 109 };
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16, cudaDevAttrComputeCapabilityMajor = 75, cudaDevAttrComputeCapabilityMinor = 76, cudaDevAttrMaxPersistingL2CacheSize = 108, cudaDevAttrMaxAccessPolicyWindowSize = 109 };
 enum cudaLimit { cudaLimitPersistingL2CacheSize = 6 };
 enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
 enum cudaAccessProperty { cudaAccessPropertyNormal = 0, cudaAccessPropertyStreaming = 1, cudaAccessPropertyPersisting = 2 };
@@ -167,7 +167,7 @@ inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) {
   switch (a) {
     case cudaDevAttrMultiProcessorCount: { const char* e = getenv("SERFSIM_EMU_SMS"); *v = e ? atoi(e) : 1; break; }
-    case cudaDevAttrComputeCapabilityMajor: *v = 10; break;
+    case cudaDevAttrComputeCapabilityMajor: *v = 9; break;          // minor: 0 (default)
     default: *v = 0;
   }
   return cudaSuccess;

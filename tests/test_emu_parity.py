@@ -248,7 +248,7 @@ def test_fuzz_with_user_events_and_injectors(seed):
         _feature_checks(g, o, sc)
 
 
-@pytest.mark.skipif(not __import__("os").environ.get("SERFSIM_SLOW"), reason="≈ 2 min and 3 GB: set SERFSIM_SLOW=1 (result recorded in profiles/r1_notes.md)")
+@pytest.mark.skipif(not __import__("os").environ.get("SERFSIM_SLOW"), reason="≈ 2 min and 3 GB: set SERFSIM_SLOW=1")
 def test_bench_workload_full_10m_nodes():
     """The bench workload itself — BASELINE configs[3] shape on one device: 10 M-node random graph, fan-out 4, one
     dissemination to quiescence — through the host-compiled kernel in production mode, against the oracle (8 threads)."""

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-kernel SASS fingerprints of serf_b200/libserfsim.so.
 
-  python tools/sass_hashes.py --write profiles/<name>.json     record the fingerprints of the current build
-  python tools/sass_hashes.py --check profiles/<name>.json     list the kernels whose machine code differs from that record
+  python tools/sass_hashes.py --write <name>.json     record the fingerprints of the current build
+  python tools/sass_hashes.py --check <name>.json     list the kernels whose machine code differs from that record
 
 Used to state precisely which kernels changed since the build a GPU parity run last passed on (source refactors that
 leave the machine code untouched — launch macros, host-only #ifdefs — show up as "no kernel changed")."""

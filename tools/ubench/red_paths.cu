@@ -1,13 +1,13 @@
-// Where does the scattered-RED floor of the tick kernel come from?  (profiles/r2a_ubench_lsu_red.txt: 4 scattered RED.MAX per
-// node = 209 us per 10 M nodes = 1.47 SM-cycles per lane — the largest share of a plateau tick.)  This benchmark separates
-//   * SM side (LSU / L1tex wavefronts) from L2 side (atomic units): the same work on 148, 74 and 37 SMs — an SM-side limit
+// Where does the scattered-RED floor of the tick kernel come from?  (4 scattered RED.MAX per node are the largest share of
+// a plateau tick.)  This benchmark separates
+//   * SM side (LSU / L1tex wavefronts) from L2 side (atomic units): the same work on 132, 66 and 33 SMs — an SM-side limit
 //     scales with the number of SMs, an L2-side limit does not;
 //   * the operation: RED.MAX vs RED.ADD vs plain scattered STG.32 vs scattered LDG.32, with / without the evict_last hint;
 //   * the footprint: a 4 MB / 40 MB plane (L2 resident) vs 240 MB (the two-slot bench workload's six planes);
 //   * occupancy: 1, 2, 4, 8 CTAs of 256 threads per SM;
 //   * locality: targets confined to a 1 MB window that moves with the node id (what a small-world graph's ring
 //     neighbours look like) vs uniformly random targets.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/ubench/red_paths tools/ubench/red_paths.cu
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/ubench/red_paths tools/ubench/red_paths.cu
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -63,7 +63,7 @@ template <int OP, int PER_NODE>
 static void run(const char* name, u32 n, u32 span, u32 window, u32* plane, u32* work, u32* sink, int ctas_per_sm, u32 sm_limit) {
   cudaEvent_t a, b;
   cudaEventCreate(&a); cudaEventCreate(&b);
-  const int grid = 148 * ctas_per_sm;
+  const int grid = 132 * ctas_per_sm;
   const int reps = 6;
   float best = 1e30f, tot = 0;
   for (int r = 0; r < reps + 2; ++r) {
@@ -93,34 +93,34 @@ int main(int argc, char** argv) {
   cudaDeviceGetAttribute(&clk_khz, cudaDevAttrClockRate, 0);
   if (clk_khz > 0) g_clk_ghz = clk_khz * 1e-6;
   printf("# n = %u nodes, 4 scattered ops per node unless stated, 256-thread CTAs, SM clock %.3f GHz (nominal max)\n", n, g_clk_ghz);
-  printf("## operation (40 MB plane, 148 SMs, 4 CTAs/SM)\n");
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 148);
-  run<OP_RED_MAX, 4>("RED.MAX", n, n, 0, plane, work, sink, 4, 148);
-  run<OP_RED_ADD, 4>("RED.ADD", n, n, 0, plane, work, sink, 4, 148);
-  run<OP_STG, 4>("STG.32", n, n, 0, plane, work, sink, 4, 148);
-  run<OP_LDG, 4>("LDG.32", n, n, 0, plane, work, sink, 4, 148);
+  printf("## operation (40 MB plane, 132 SMs, 4 CTAs/SM)\n");
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 132);
+  run<OP_RED_MAX, 4>("RED.MAX", n, n, 0, plane, work, sink, 4, 132);
+  run<OP_RED_ADD, 4>("RED.ADD", n, n, 0, plane, work, sink, 4, 132);
+  run<OP_STG, 4>("STG.32", n, n, 0, plane, work, sink, 4, 132);
+  run<OP_LDG, 4>("LDG.32", n, n, 0, plane, work, sink, 4, 132);
   printf("## SM count (RED.MAX evict_last, 40 MB plane, 4 CTAs/SM): SM-side limit scales, L2-side limit does not\n");
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 111);
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 74);
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 37);
-  run<OP_STG, 4>("STG.32", n, n, 0, plane, work, sink, 4, 74);
-  run<OP_LDG, 4>("LDG.32", n, n, 0, plane, work, sink, 4, 74);
-  printf("## occupancy (RED.MAX evict_last, 40 MB plane, 148 SMs)\n");
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 1, 148);
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 2, 148);
-  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 8, 148);
-  printf("## footprint (RED.MAX evict_last, 148 SMs, 4 CTAs/SM)\n");
-  run<OP_RED_MAX_HINT, 4>("4 MB plane", n, 1000000u, 0, plane, work, sink, 4, 148);
-  run<OP_RED_MAX_HINT, 4>("80 MB", n, 20000000u, 0, plane, work, sink, 4, 148);
-  run<OP_RED_MAX_HINT, 4>("120 MB", n, 30000000u, 0, plane, work, sink, 4, 148);
-  run<OP_RED_MAX_HINT, 4>("240 MB", n, big, 0, plane, work, sink, 4, 148);
-  run<OP_RED_MAX, 4>("240 MB, no hint", n, big, 0, plane, work, sink, 4, 148);
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 99);
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 66);
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 4, 33);
+  run<OP_STG, 4>("STG.32", n, n, 0, plane, work, sink, 4, 66);
+  run<OP_LDG, 4>("LDG.32", n, n, 0, plane, work, sink, 4, 66);
+  printf("## occupancy (RED.MAX evict_last, 40 MB plane, 132 SMs)\n");
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 1, 132);
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 2, 132);
+  run<OP_RED_MAX_HINT, 4>("RED.MAX evict_last", n, n, 0, plane, work, sink, 8, 132);
+  printf("## footprint (RED.MAX evict_last, 132 SMs, 4 CTAs/SM)\n");
+  run<OP_RED_MAX_HINT, 4>("4 MB plane", n, 1000000u, 0, plane, work, sink, 4, 132);
+  run<OP_RED_MAX_HINT, 4>("80 MB", n, 20000000u, 0, plane, work, sink, 4, 132);
+  run<OP_RED_MAX_HINT, 4>("120 MB", n, 30000000u, 0, plane, work, sink, 4, 132);
+  run<OP_RED_MAX_HINT, 4>("240 MB", n, big, 0, plane, work, sink, 4, 132);
+  run<OP_RED_MAX, 4>("240 MB, no hint", n, big, 0, plane, work, sink, 4, 132);
   printf("## locality (RED.MAX evict_last, 40 MB plane): targets within a window around the sender's own index\n");
-  run<OP_RED_MAX_HINT, 4>("window 1 MB (256 K words)", n, n, 262144u, plane, work, sink, 4, 148);
-  run<OP_RED_MAX_HINT, 4>("window 64 KB (16 K words)", n, n, 16384u, plane, work, sink, 4, 148);
-  run<OP_RED_MAX_HINT, 4>("window 4 KB (1 K words)", n, n, 1024u, plane, work, sink, 4, 148);
+  run<OP_RED_MAX_HINT, 4>("window 1 MB (256 K words)", n, n, 262144u, plane, work, sink, 4, 132);
+  run<OP_RED_MAX_HINT, 4>("window 64 KB (16 K words)", n, n, 16384u, plane, work, sink, 4, 132);
+  run<OP_RED_MAX_HINT, 4>("window 4 KB (1 K words)", n, n, 1024u, plane, work, sink, 4, 132);
   printf("## ops per node (RED.MAX evict_last, 40 MB plane)\n");
-  run<OP_RED_MAX_HINT, 1>("1 per node", n, n, 0, plane, work, sink, 4, 148);
-  run<OP_RED_MAX_HINT, 8>("8 per node", n, n, 0, plane, work, sink, 4, 148);
+  run<OP_RED_MAX_HINT, 1>("1 per node", n, n, 0, plane, work, sink, 4, 132);
+  run<OP_RED_MAX_HINT, 8>("8 per node", n, n, 0, plane, work, sink, 4, 132);
   return 0;
 }
