@@ -92,6 +92,7 @@ struct serfsim {
   u8* d_hot[2] = {nullptr, nullptr};      // [n_tiles] per tick parity
   u8* d_hot_static = nullptr;             // [n_tiles] tiles that hold a watcher (never consumed)
   u32* d_node_due = nullptr;              // [stride] per-node earliest suspicion deadline (tick_kernel.cuh)
+  u32* d_carry = nullptr;                 // [stride] per-view passes: carry words (tick_kernel.cuh: CARRY_*); unsharded multi-slot runs only
   u32* d_tile_due = nullptr;              // [n_tiles] earliest suspicion deadline of a tile's nodes (the timer wheel)
   u32* d_sched = nullptr;                 // scheduler words (tick_kernel.cuh: SCHED_*)
   u32 n_tiles = 0;
@@ -134,7 +135,7 @@ struct serfsim {
   std::vector<u32> subj;
   u32 up_mask = 0;
   u32 ever_down = 0;               // subjects that have been down at some tick since the reset (only those are probed, suspected, run timers)
-  u32 sv = 1;                      // single-view ticks of multi-slot runs: 1 = dual launch, 2 = check mode, 0 = off (SERFSIM_SV, tick_kernel.cuh)
+  u32 sv = 1;                      // multi-slot runs: 1 = per-view passes (sharded: single-view dual launch), 2 = check mode, 0 = off (SERFSIM_SV, tick_kernel.cuh)
   int grid_sv = 0;                 // grid of the single-view kernel
   u32 tick = 0;
   bool has_topo = false;
@@ -338,17 +339,35 @@ int launch_ticks(serfsim* h, u32 n) {
       launch_uevent(u, h->cfg.trace != 0, h->stream);
       h->last_launches++;
     }
-    // Multi-slot runs in production mode: the general kernel and the single-view kernel are both launched, the device decides (SV_*)
-    const bool sv_ok = h->sv && h->R > 1 && h->R < 32 && !h->cfg.trace && p.sleep_on && !h->byz_on && __builtin_popcount(h->ever_down) == 1;
-    if (sv_ok) {
+    // Multi-slot runs in production mode (SV_*, tick_kernel.cuh).  Unsharded: ticks without a host operation or a reaper round run as
+    // per-view passes of the single-slot kernel.  Sharded: while exactly one subject has ever been down, the general kernel and the
+    // single-view kernel are both launched and the device decides.
+    const bool sv_ok = h->sv && h->R > 1 && h->R < 32 && !h->cfg.trace && p.sleep_on && !h->byz_on;
+    const bool pass_tick = sv_ok && !sharded && ee == eb && !p.reap_now && t + 1 < CARRY_TICKS;
+    const bool dual = sv_ok && sharded && __builtin_popcount(h->ever_down) == 1;
+    if (pass_tick || dual) {
       const bool all = ee > eb || p.reap_now;                 // a host operation or a reaper round visits every view
       p.views_host = all ? 0xffffffffu : h->ever_down;
       p.sv_mode = h->sv == 2 ? SV_CHECK : SV_GENERAL;
-      p.sv_slot = (u32)__builtin_ctz(h->ever_down); p.sv_R = h->R;
+      p.sv_slot = h->ever_down ? (u32)__builtin_ctz(h->ever_down) : 0u; p.sv_R = h->R;
     }
-    launch_tick(p, h->cfg.trace != 0, h->grid, h->stream);
-    h->last_launches++;
-    if (sv_ok && h->sv == 1) {
+    if (pass_tick && h->sv == 1) {
+      p.sv_mode = SV_PASS; p.carry = h->d_carry;
+      p.tiles_per_cta = (h->n_tiles + h->grid_sv - 1) / h->grid_sv;
+      for (u32 s0 = 0; s0 < h->R; ++s0) {                  // ascending slot order: what the view loop carries from view to view travels through memory
+        TickParams q = p;                                  // the planes as the single-slot kernel sees them: they start at view s0
+        q.gate.evaluate = s0 == 0 ? p.gate.evaluate : 0u; q.sv_wshift = s0; q.sv_slot = s0;
+        q.rec = p.rec + 2 * (size_t)s0 * h->stride; q.qword = p.qword + (size_t)s0 * h->stride;
+        q.inbox_rd = p.inbox_rd + (size_t)s0 * h->stride; q.inbox_wr = p.inbox_wr + (size_t)s0 * h->stride;
+        q.subj[0] = p.subj[s0]; q.down_mask = (p.down_mask >> s0) & 1u;
+        launch_tick_pass(q, h->grid_sv, h->stream);
+        h->last_launches++;
+      }
+    } else {
+      launch_tick(p, h->cfg.trace != 0, h->grid, h->stream);
+      h->last_launches++;
+    }
+    if (dual && h->sv == 1) {
       TickParams q = p;                                    // the planes as the single-slot kernel sees them: they start at view sv_slot
       const u32 s0 = p.sv_slot;
       q.sv_mode = SV_SINGLE; q.gate.evaluate = 0u; q.sv_wshift = s0;
@@ -562,6 +581,7 @@ int do_reset(serfsim* h, u64 seed) {
   CU(cudaMemsetAsync(h->d_hot[1], 0, h->n_tiles, h->stream));
   CU(cudaMemsetAsync(h->d_tile_due, 0xff, (size_t)h->n_tiles * sizeof(u32), h->stream));      // no timer runs
   CU(cudaMemsetAsync(h->d_node_due, 0xff, (size_t)h->stride * sizeof(u32), h->stream));
+  if (h->d_carry) CU(cudaMemsetAsync(h->d_carry, 0, (size_t)h->stride * sizeof(u32), h->stream));   // tags restart with the ticks
   CU(cudaMemsetAsync(h->d_sched, 0, SCHED_WORDS * sizeof(u32), h->stream));
   if (h->d_trace) {
     CU(cudaMemsetAsync(h->d_trace, 0, (size_t)h->trace_cap * 8 * sizeof(u64), h->stream));
@@ -580,7 +600,7 @@ int do_reset(serfsim* h, u64 seed) {
 void free_all(serfsim* h) {
   for (void* p : h->ipc_opened) cudaIpcCloseMemHandle(p);
   for (cudaEvent_t e : h->tick_ev) cudaEventDestroy(e);
-  cudaFree(h->d_hot_static); cudaFree(h->d_tile_due); cudaFree(h->d_node_due); cudaFree(h->d_sched);
+  cudaFree(h->d_hot_static); cudaFree(h->d_tile_due); cudaFree(h->d_node_due); cudaFree(h->d_carry); cudaFree(h->d_sched);
   cudaFree(h->d_hot[0]); cudaFree(h->d_hot[1]); cudaFree(h->d_busy); cudaFree(h->d_watch); cudaFree(h->d_snap_rec); cudaFree(h->d_snap_node); cudaFree(h->d_peer_snap_rec); cudaFree(h->d_peer_snap_node);
   cudaFree(h->d_qword);
   cudaFree(h->d_rec); cudaFree(h->d_inbox[0]); cudaFree(h->d_inbox[1]); cudaFree(h->d_node); cudaFree(h->d_rowptr); cudaFree(h->d_col);
@@ -705,6 +725,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   CUB(cudaMalloc(&h->d_hot[0], h->n_tiles)); CUB(cudaMalloc(&h->d_hot[1], h->n_tiles));
   CUB(cudaMalloc(&h->d_hot_static, h->n_tiles)); CUB(cudaMalloc(&h->d_tile_due, (size_t)h->n_tiles * sizeof(u32))); CUB(cudaMalloc(&h->d_node_due, (size_t)h->stride * sizeof(u32))); CUB(cudaMalloc(&h->d_sched, SCHED_WORDS * sizeof(u32)));
   CUB(cudaMemset(h->d_hot_static, 0, h->n_tiles));
+  if (h->R > 1 && cfg->world_size <= 1) CUB(cudaMalloc(&h->d_carry, (size_t)h->stride * sizeof(u32)));
   CUB(cudaHostAlloc(&h->pin_overflow, sizeof(u32), cudaHostAllocMapped));
   CUB(cudaHostGetDevicePointer(&h->d_overflow, h->pin_overflow, 0));
   *h->pin_overflow = 0;

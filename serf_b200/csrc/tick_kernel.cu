@@ -350,7 +350,12 @@ __device__ __forceinline__ u32 pick_finish(u32 v, const u32 (&cand)[FMAX], u32 (
 // bit 3 some view of the node runs a suspicion timer (it sleeps until its tile comes due, tick_kernel.cuh).
 // nd: the node's own earliest suspicion deadline (node_due), read only in tiles that have come due
 struct Pre { u32 busy, mL, mJ, mM, any, qw, mailmask, qmask, keep, nd; };   // mL, mJ, mM, qw: the words of view `keep` (0 in single-slot runs)
-template <bool R1>
+// Carry word of node vl in this tick (CARRY_*), 0 when no earlier pass of the tick visited it.
+__device__ __forceinline__ u32 carry_of(const TickParams& p, u32 vl) {
+  const u32 w = p.carry[vl];
+  return (w >> 8) == ((p.tick + 1u) & (CARRY_TICKS - 1u)) ? (w & 0xffu) : 0u;
+}
+template <bool R1, bool PASS = false>
 __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool kL, bool kJ, bool kM, u64 pol_first, bool due, u32 keep = 0) {
   // R1: the kernel visits exactly one view, the one its planes start with (single-slot runs; single-view ticks of multi-slot runs, whose
   // parameter block points at the active view — the distance between the planes of two kinds is p.R views either way)
@@ -371,6 +376,9 @@ __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool k
     x.mailmask |= ((l | j | m) ? 1u : 0u) << s2;
     x.qmask |= (q ? 1u : 0u) << s2;
   }
+  // A pass cannot trust busy bits 0 and 3 (an earlier pass of the tick rewrote them): a queued transmit is business of the view itself,
+  // and a node whose timers were due when the tick began visits every view (`any` stands for both in the activity test).
+  if (PASS) x.any |= x.qw | ((due && (carry_of(p, vl) & CARRY_TDUE)) ? 1u : 0u);
   return x;
 }
 // Has the node anything to do this tick?  (due: its tile's earliest suspicion deadline has been reached — then a node that runs timers
@@ -475,10 +483,12 @@ __device__ SFS_COLD bool cold_can_confirm(u32 k, u32 mask, u32 v) {
 // A view whose only business is a running suspicion timer does not: its deadline goes to `mind` (the caller registers the
 // minimum in tile_due) and the view sleeps until its tile comes due.  `due`: this tile's earliest deadline has been reached —
 // every node of it that carries a timer (busy bit 3) visits all its views.
-template <bool TRACE, int FMAX, bool SHARDED, bool R1, bool STAGED>
+template <bool TRACE, int FMAX, bool SHARDED, bool R1, bool STAGED, bool PASS = false>
 __device__ __forceinline__ bool process_node(const TickParams& p, const StageView& sv, XStage* xs, const u32 vl, const Pre& pre, const bool kL, const bool kJ, const bool kM, const bool mark, const bool saturated,
-                                             const bool due, const u64 pol_first, const u64 pol_last, Counters& c, u32& mind, int& dsusp, const Ahead<FMAX>& ah, u32& first_view, const u32 sv_views = 0xffffffffu) {
+                                             const bool due, const u64 pol_first, const u64 pol_last, Counters& c, u32& mind, int& dsusp, const Ahead<FMAX>& ah, u32& first_view, const u32 sv_views = 0xffffffffu,
+                                             const bool carry_out = false) {
   static_assert(!STAGED || R1, "the staged path is the single-slot path");
+  static_assert(!PASS || (R1 && !STAGED && !SHARDED && !TRACE), "passes are single-slot kernels of unsharded production runs");
   const u32 lt = threadIdx.x;              // index inside the staged tile
   const u32 v = p.first + vl;
   const u32 t = p.tick;
@@ -518,8 +528,11 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   u32 nd = pre.nd;                                       // the node's own earliest deadline: matters in due tiles, for nodes that run timers
   if (R1 && due && (busy & 8u)) nd = p.node_due[vl];
   const u32 sleeping = (due && (busy & 8u)) ? nd : NO_DEADLINE;
-  const bool timers_due = sleeping <= p.tick;
+  bool timers_due = sleeping <= p.tick;
+  u32 cr = 0;                                            // PASS: what the earlier passes of this tick did at this node
+  if (PASS && due) { cr = carry_of(p, vl); if (cr & CARRY_SEEN) timers_due = (cr & CARRY_TDUE) != 0; }   // as it was when the tick began
   if (!TRACE && !STAGED && !((busy & 7u) != 0 || pre.any != 0 || p.reap_now != 0 || timers_due)) { mind = min(mind, sleeping); if (due && (busy & 8u)) SFS_PROBE(20); return false; }
+  if (PASS && !due) cr = carry_of(p, vl);
   if (STAGED && !TRACE && !((busy & 7u) || (mL | mJ | mM) || p.reap_now || timers_due)) { mind = min(mind, sleeping); return false; }
   // (the watcher mask — subjects this node can probe, it has them as neighbours — is re-read where a watcher needs it: a handful of nodes)
 #define SFS_WMASK() ((busy & 4u) ? ((u32)p.watch[vl] >> p.sv_wshift) : 0u)   /* sv_wshift: the view a single-view launch works on (0 in every other launch) */
@@ -669,7 +682,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
       // noticed yet.  Suspect views are counted by the persistent counter (they sleep), the others here.  A watcher's view of
       // a down subject stays awake while it is Alive or Suspect: its own failed probe may still start or confirm the suspicion.
       const bool queued = (r.txl | r.txj | r.txm) != 0;
-      if (!R1 && (queued || mx)) c.views |= 1u << s;                  // the view sent mail or keeps a queue: it has business in the next tick (single-view ticks)
+      if ((!R1 || PASS) && (queued || mx)) c.views |= 1u << (s + p.sv_slot * PASS);   // the view sent mail or keeps a queue: it has business in the next tick (passes, single-view ticks)
       const bool watching = (busy & 4u) && p.probe_every && ((p.down_mask >> s) & 1) && !self && ((SFS_WMASK() >> s) & 1);
       const bool suspect = r.mlstate == ML_SUSPECT;
       { const u32 pnd = (!suspect && (queued || (watching && r.mlstate == ML_ALIVE))) ? 1u : 0u; if (R1) c.cp += pnd << 16; else c.pending += pnd; }
@@ -697,21 +710,32 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   if (ns2 != ns) st_u64_stream(p.node_state + vl, ns2, pol_first);
   if (TRACE) c.hash += node_hash((u64)R * p.n_global + v, ns2);
   if (clock >= LTIME_LIMIT) *p.overflow = 1;
-  if (R1) c.pe += min(nt, max_tx); else c.packets += min(nt, max_tx);
+  // packets: min(#peers, the largest budget of any view) — a pass counts what the earlier passes of the tick have not
+  const u32 pk = min(nt, max_tx), pk_before = PASS ? (cr & CARRY_PK) : 0u;
+  if (R1) c.pe += pk > pk_before ? pk - pk_before : 0u; else c.packets += pk;
+  const bool awake_node = awake || (PASS && (cr & CARRY_AWAKE));
+  // What a visit of every view makes exact.  A pass sees every view of a node whose timers were due only together with the other passes
+  // of the tick: the first pass that visits it writes exactly, the later ones add to what it wrote.
+  const bool exact = PASS ? (timers_due && !(cr & CARRY_SEEN)) : visit_all;
   // busy byte: the op bit is consumed, the watcher bit is static; the timer bit is exact after a visit of every view and
   // sticky otherwise (a view that was not visited may run a timer: it is found when its tile comes due)
-  const u32 busy2 = (awake ? 1u : 0u) | (busy & 4u) | ((has_timer || (!visit_all && (busy & 8u))) ? 8u : 0u);
+  const u32 busy2 = (awake_node ? 1u : 0u) | (busy & 4u) | ((has_timer || (!exact && (busy & 8u))) ? 8u : 0u);
   if (busy2 != busy) p.busy[vl] = (u8)busy2;
   // node_due: a lower bound of the node's earliest running deadline, exact after a visit of every view.  A view's deadline only moves
-  // while the view is visited, so views that were not visited are still covered by the word as it stands.
+  // while the view is visited, so views that were not visited are still covered by the word as it stands (in a pass: unless an earlier
+  // pass rewrote the word exactly).
   if (has_timer) {
-    if (visit_all || !(busy & 8u)) p.node_due[vl] = mind;
-    else if (dl_moved) atomicMin(p.node_due + vl, mind);
+    if (exact || !(busy & 8u)) p.node_due[vl] = mind;
+    else if (dl_moved || (PASS && (cr & CARRY_TDUE))) atomicMin(p.node_due + vl, mind);
   }
-  if (!visit_all) mind = min(mind, sleeping);   // its tile's entry was reset: timers of the views not visited go back with the node's word
+  if (PASS ? !timers_due : !visit_all) mind = min(mind, sleeping);   // its tile's entry was reset: timers of the views not visited go back with the node's word
+  if (PASS && carry_out)                                 // a later pass of this tick has business
+    p.carry[vl] = (((p.tick + 1u) & (CARRY_TICKS - 1u)) << 8) | CARRY_SEEN | (timers_due ? CARRY_TDUE : 0u) | (awake_node ? CARRY_AWAKE : 0u) | max(pk, pk_before);
   // The scheduler must know whether anybody stays awake.  A node that sent a packet this tick shows in the row's message count;
   // the others (a watcher on probe duty, a queue that has no peer to go to, a transmit queued after the send phase) are rare.
-  if (awake && min(nt, max_tx) == 0) atomicAdd(p.sched + SCHED_AWAKE, 1u);
+  // (a pass counts the node when its own view leaves it awake without a packet: more often than the view loop would only if a packet was
+  // sent in the tick, and then the row's message count keeps the cluster awake anyway)
+  if (awake && pk == 0) atomicAdd(p.sched + SCHED_AWAKE, 1u);
   return awake;
 }
 
@@ -746,13 +770,23 @@ __device__ __forceinline__ void write_idle_row(const TickParams& p) {
 
 // Scan of the CTA's tile flags.  hot_s[i]: bit 0 = process the tile, bit 1 = its earliest suspicion deadline has been reached
 // (the entry is reset here, by the tile's owner, before any of its nodes runs: the timers that are still running re-register).
-__device__ __forceinline__ void scan_tiles(const TickParams& p, u8* hot_s, u32 tile0, u32 ntile, bool all_hot) {
+// keep (first of several passes): the flags are replaced by the decision instead of being consumed; the later passes read it (tile_decisions).
+__device__ __forceinline__ void scan_tiles(const TickParams& p, u8* hot_s, u32 tile0, u32 ntile, bool all_hot, bool keep = false) {
   for (u32 i = threadIdx.x; i < ntile; i += BLOCK) {
     const u8 f = p.hot_rd[tile0 + i];
-    if (f) p.hot_rd[tile0 + i] = 0;                      // consumed; this parity is written again two ticks from now
     const bool due = p.tile_due[tile0 + i] <= p.tick;
     if (due) { p.tile_due[tile0 + i] = NO_DEADLINE; SFS_PROBE(4); }     // tiles woken by the timer wheel
-    hot_s[i] = (u8)(((f || all_hot || due || p.hot_static[tile0 + i]) ? 1u : 0u) | (due ? 2u : 0u));
+    const u8 d = (u8)(((f || all_hot || due || p.hot_static[tile0 + i]) ? 1u : 0u) | (due ? 2u : 0u));
+    hot_s[i] = d;
+    if (keep ? d != f : f != 0) p.hot_rd[tile0 + i] = keep ? d : 0;   // consumed; this parity is written again two ticks from now
+  }
+}
+// Later passes of a tick: the first pass's decision (nothing to process for a pass without business); the last pass consumes it.
+__device__ __forceinline__ void tile_decisions(const TickParams& p, u8* hot_s, u32 tile0, u32 ntile, bool last, bool work) {
+  for (u32 i = threadIdx.x; i < ntile; i += BLOCK) {
+    const u8 d = p.hot_rd[tile0 + i];
+    hot_s[i] = work ? d : (u8)0;
+    if (last && d) p.hot_rd[tile0 + i] = 0;
   }
 }
 
@@ -776,7 +810,7 @@ __device__ __forceinline__ void publish_to_peer(u32 r, u32 world, u32 rank, u32 
 // End of a tick: block reduction of the counters (warp shuffles, then shared memory) → one atomic per counter per CTA; the
 // LAST CTA to finish (ticket) completes the row and decides how long the cluster can sleep.
 // trace row: 0 packets, 1 edge_updates, 2 messages, 3 changed, 4 pending, (5 events, 6 suspects: direct), 7 hash
-template <bool TRACE, bool PACKED>
+template <bool TRACE, bool PACKED, bool PASS = false>
 __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters& c, u64 (*red)[BLOCK / 32], int dsusp_cta) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   __shared__ u32 last_s, due_min_s[BLOCK / 32];
@@ -803,6 +837,7 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
   }
   if (TRACE && lane == 0 && hs) atomicAdd((unsigned long long*)(p.row + 7), (unsigned long long)hs);
   { const u32 vw = __reduce_or_sync(0xffffffffu, c.views); if (lane == 0 && vw) atomicOr(p.sched + SCHED_VIEWS_NEXT, vw); }
+  if (PASS && p.sv_slot + 1u < p.sv_R) return;             // the last pass of the tick completes it
   // ---- ticket: every CTA's counters are in the row before the last one reads it ----
   __threadfence();
   __syncthreads();
@@ -866,7 +901,7 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
 // "hot": somebody delivered into it during the previous tick, it holds a node that stays awake (queued transmits,
 // probe duty), a host operation targets it, or a suspicion timer of one of its nodes has come due — otherwise not a
 // single byte of it is touched.
-template <bool TRACE, int FMAX, bool SHARDED, bool R1, int MB>
+template <bool TRACE, int FMAX, bool SHARDED, bool R1, int MB, bool PASS = false>
 __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__ TickParams p) {
   __shared__ u8 hot_s[MAX_TILES_PER_CTA];
   __shared__ u64 red[8][BLOCK / 32];
@@ -874,18 +909,26 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   __shared__ __align__(16) unsigned char xs_mem[SHARDED ? sizeof(XStage) : 16];
   XStage* xs = reinterpret_cast<XStage*>(xs_mem);
   if (gate_closed(p.gate, blockIdx.x == 0 && threadIdx.x == 0)) return;   // the run is over (uniform over the grid): this tick does not exist
-  if (tick_is_idle(p.sched, p.tick, p.ev_begin, p.ev_end)) { if (p.sv_mode != SV_SINGLE) write_idle_row<TRACE>(p); return; }   // nothing can happen in this tick (uniform)
+  if (tick_is_idle(p.sched, p.tick, p.ev_begin, p.ev_end)) { if (PASS ? p.sv_slot == 0 : p.sv_mode != SV_SINGLE) write_idle_row<TRACE>(p); return; }   // nothing can happen in this tick (uniform)
   // Single-view ticks of multi-slot runs (tick_kernel.cuh, SV_*): the general kernel and the single-view kernel are both launched; the
   // set of views that can have business in this tick — known on the device since the end of the previous tick — decides which one runs.
   u32 sv_views = 0xffffffffu;
-  if (p.sv_mode != SV_OFF) {
+  bool work = true, carry_out = false;                     // PASS: this pass's view has business; so has a later pass's
+  if (PASS) {
+    const u32 sv_base = p.tick >= p.sched[SCHED_VIEWS_FROM] ? p.sched[SCHED_VIEWS_NEW] : p.sched[SCHED_VIEWS_OLD];
+    const u32 views = (sv_base | p.views_host) & ((1u << p.sv_R) - 1u);
+    work = (views >> p.sv_slot) & 1u;
+    carry_out = (views >> p.sv_slot) > 1u;
+    if (work) SFS_PROBE(21);
+    else if (p.sv_slot != 0 && p.sv_slot + 1u < p.sv_R) return;    // neither node work nor a duty of the first or the last pass
+  } else if (p.sv_mode != SV_OFF) {
     // (the kernel of this tick that ran before this one, if any, has already published the NEXT tick's set: SCHED_VIEWS_FROM says since when it holds)
     const u32 sv_base = p.tick >= p.sched[SCHED_VIEWS_FROM] ? p.sched[SCHED_VIEWS_NEW] : p.sched[SCHED_VIEWS_OLD];
     const u32 views = (sv_base | p.views_host) & ((1u << p.sv_R) - 1u);
     const bool single = views == (1u << p.sv_slot);        // exactly the one view the single-view launch was set up for
     if (p.sv_mode == SV_SINGLE) { if (!single) return; SFS_PROBE(21); }
     else if (p.sv_mode == SV_GENERAL && single) return;
-    if (p.sv_mode == SV_CHECK && single) sv_views = views;   // checked only where the single-view kernel would have run
+    if (p.sv_mode == SV_CHECK && (single || p.world == 1)) sv_views = views;   // checked where the single-view kernel or the passes would have run
   }
   if (threadIdx.x == 0) dsusp_s = 0;                       // ordered before its first use by the barrier after the tile scan
   Counters c = {};
@@ -910,8 +953,9 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   const u32 tile0 = blockIdx.x * p.tiles_per_cta;
   const u32 ntile = tile0 < p.n_tiles ? min(p.tiles_per_cta, p.n_tiles - tile0) : 0;
   if (SHARDED && saturated && ntile && (u32)lane < p.world && (u32)lane != p.rank) { resv = atomicAdd(p.send_count + lane, XW_FLUSH); rlen = XW_FLUSH; }   // every warp will send to every peer
-  scan_tiles(p, hot_s, tile0, ntile, all_hot);
+  if (PASS && p.sv_slot != 0) tile_decisions(p, hot_s, tile0, ntile, p.sv_slot + 1u == p.sv_R, work); else scan_tiles(p, hot_s, tile0, ntile, all_hot, PASS);
   __syncthreads();
+  if (PASS && !work && p.sv_slot + 1u < p.sv_R) return;   // the first pass without business has made the tiles' decisions
   // Unsaturated ticks (ramp-up and tail of a dissemination: a few per cent of the nodes have anything to do, spread
   // one or two per warp): a tile-by-tile walk pays one chain of dependent round trips (state → row → peers) per TILE
   // for a handful of active lanes.  Instead the CTA scans GROUP hot tiles at once — the 13 "anything to do?" bytes
@@ -939,7 +983,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
         pr[g] = Pre{};
         if (g < ng) {
           const u32 vn = ((tile0 + gt_s[g]) << TILE_SHIFT) + threadIdx.x;
-          if (vn < p.n_local) pr[g] = prefetch_node<R1>(p, vn, kL, kJ, kM, pol_first, false);   // (a node's own deadline is read below, in due tiles only: eight more live registers otherwise)
+          if (vn < p.n_local) pr[g] = prefetch_node<R1, PASS>(p, vn, kL, kJ, kM, pol_first, PASS && (hot_s[gt_s[g]] & 2u) != 0);   // (a node's own deadline is read below, in due tiles only: eight more live registers otherwise)
         }
       }
 #pragma unroll
@@ -980,11 +1024,11 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
             pre.mailmask = pre.any ? 1u : 0u; pre.qmask = pre.qw ? 1u : 0u;
             SFS_COUNT(6, 4);
           } else {
-            pre = prefetch_node<R1>(p, vl, kL, kJ, kM, pol_first, (hot_s[ti] & 2u) != 0);   // per-view masks are not carried through the list: the few active nodes read them again
+            pre = prefetch_node<R1, PASS>(p, vl, kL, kJ, kM, pol_first, (hot_s[ti] & 2u) != 0);   // per-view masks are not carried through the list: the few active nodes read them again
           }
           u32 mind = NO_DEADLINE, fv_unused = 0;
           int dsusp = 0;
-          const bool pend = process_node<TRACE, FMAX, SHARDED, R1, false>(p, StageView{}, xs, vl, pre, kL, kJ, kM, mark, false, (hot_s[ti] & 2u) != 0, pol_first, pol_last, c, mind, dsusp, Ahead<FMAX>{}, fv_unused, sv_views);
+          const bool pend = process_node<TRACE, FMAX, SHARDED, R1, false, PASS>(p, StageView{}, xs, vl, pre, kL, kJ, kM, mark, false, (hot_s[ti] & 2u) != 0, pol_first, pol_last, c, mind, dsusp, Ahead<FMAX>{}, fv_unused, sv_views, carry_out);
           if (mark && pend) pend_s[g] = 1;
           if (mind != NO_DEADLINE) atomicMin(p.tile_due + tile0 + ti, mind);      // the list mixes tiles: per-lane registration (few active nodes)
           if (dsusp) atomicAdd(&dsusp_s, dsusp);
@@ -1003,7 +1047,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   u32 first_view = 0;                                      // the first view this thread visited in its last tile
   auto prefetch_tile = [&](u32 ti) -> Pre {
     const u32 vn = ((tile0 + ti) << TILE_SHIFT) + threadIdx.x;
-    return vn < p.n_local ? prefetch_node<R1>(p, vn, kL, kJ, kM, pol_first, (hot_s[ti] & 2u) != 0, first_view) : Pre{};
+    return vn < p.n_local ? prefetch_node<R1, PASS>(p, vn, kL, kJ, kM, pol_first, (hot_s[ti] & 2u) != 0, first_view) : Pre{};
   };
   auto ahead_tile = [&](u32 ti, u32 keep) -> Ahead<FMAX> {
     Ahead<FMAX> a = {};
@@ -1032,7 +1076,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
     bool pend = false;
     u32 mind = NO_DEADLINE;
     int dsusp = 0;
-    if (vl < p.n_local) pend = process_node<TRACE, FMAX, SHARDED, R1, false>(p, StageView{}, xs, vl, pre, kL, kJ, kM, mark, saturated, (hot_s[i] & 2u) != 0, pol_first, pol_last, c, mind, dsusp, ah, first_view, sv_views);
+    if (vl < p.n_local) pend = process_node<TRACE, FMAX, SHARDED, R1, false, PASS>(p, StageView{}, xs, vl, pre, kL, kJ, kM, mark, saturated, (hot_s[i] & 2u) != 0, pol_first, pol_last, c, mind, dsusp, ah, first_view, sv_views, carry_out);
     if (mark && __any_sync(0xffffffffu, pend) && lane == 0) p.hot_wr[tile0 + i] = 1;
     note_timers(p, tile0 + i, mind, dsusp, &dsusp_s);
     if (SHARDED) wrote_remote |= flush_xwarp(p, xs, false, resv, rlen);
@@ -1044,7 +1088,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
     if (wrote_remote) __threadfence_system();            // peer-window stores are performed before the publish kernel raises the flags
   }
   __syncthreads();
-  finish_tick<TRACE, R1>(p, c, red, dsusp_s);
+  finish_tick<TRACE, R1, PASS>(p, c, red, dsusp_s);
 }
 
 #ifndef SERFSIM_EMU   // the TMA pipeline is device-only (bulk copies, mbarriers); the host build of tests/emu uses the direct-load kernel
@@ -1582,7 +1626,12 @@ void launch_tick(const TickParams& p, bool trace, int grid, cudaStream_t st) {
   if (trace) { if (small) launch_tick_v<true, 4>(p, grid, st); else launch_tick_v<true, 8>(p, grid, st); }
   else { if (small) launch_tick_v<false, 4>(p, grid, st); else launch_tick_v<false, 8>(p, grid, st); }
 }
-// The single-view kernel of a dual launch (SV_SINGLE): the single-slot kernel on the one view that has business (multi-slot plane layout).
+// One pass of a tick of an unsharded multi-slot run (SV_PASS): the single-slot kernel on the view the parameter block starts at.
+void launch_tick_pass(const TickParams& p, int grid, cudaStream_t st) {
+  if (p.fanout <= 4) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 4, false, true, SFS_MB_R1, true>)(p);
+  else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 8, false, true, SFS_MB_R1, true>)(p);
+}
+// The single-view kernel of a dual launch of a sharded run (SV_SINGLE): the single-slot kernel on the one view that has business (multi-slot plane layout).
 void launch_tick_single_view(const TickParams& p, int grid, cudaStream_t st) {
   const bool sharded = p.world > 1;
   if (p.fanout <= 4) {

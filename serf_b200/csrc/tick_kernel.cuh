@@ -128,22 +128,33 @@ struct TickParams {
   u32 sv_mode, views_host, sv_slot, sv_R;    // single-view ticks (SV_*, below): sv_slot = the view the single-view launch works on, sv_R = number of views of the run
   u32 ahead;                  // multi-slot runs: 1 = saturated ticks request node word, peers and the probable first view's record one tile ahead; 2 = every tick (tests); 0 = off (SERFSIM_AHEAD)
   u32* host_idle_until;       // SCHED_IDLE_UNTIL mirrored into mapped pinned host memory: serfsim_run_until_converged does not even launch the ticks the cluster sleeps through
+  u32* carry;                 // [stride] per-view passes (SV_PASS): what the earlier passes of the tick did at the node (CARRY_*)
 };
 constexpr u32 SCHED_TICKET = 0, SCHED_IDLE_UNTIL = 1, SCHED_UE_ACTIVITY = 2, SCHED_AWAKE = 3, SCHED_SUSPECTS = 4 /* u64 */,
               SCHED_LOCAL_QUIET = 6, SCHED_LOCAL_UNTIL = 7 /* sharded runs: this rank's verdict; the drain kernel combines the ranks' */,
               SCHED_VIEWS_NEW = 8 /* single-view ticks: bit s = view s can have business, in the ticks from SCHED_VIEWS_FROM on */, SCHED_VIEWS_NEXT = 9 /* being collected */,
               SCHED_VIEWS_OLD = 10 /* the set of the tick before SCHED_VIEWS_FROM */, SCHED_VIEWS_FROM = 11, SCHED_WORDS = 12;
-// Single-view ticks (multi-slot runs).  In long stretches of a study exactly one tracked subject is in motion (the suspicion and dead waves
-// of a crash after the leave wave has died down): every node visits the same single view, and the lean single-slot kernel (80 registers,
-// 24 warps per SM, every load requested up front) does that tick faster than the multi-slot kernel (one CTA of 8 warps per SM).
+// Per-view passes (multi-slot runs).  The lean single-slot kernel (80 registers, 24 warps per SM, every load requested up front) does a
+// view's work faster than the multi-slot kernel (one CTA of 8 warps per SM), whose view loop also spreads its RED.MAX over the inbox planes
+// of every active view at once (40 MB each at 10 M nodes: two of them no longer fit the 50 MB L2).
 // Which views can have business in tick t+1 is known at the end of tick t: views that sent mail or keep a queue (collected by the tick
-// kernel, the anti-entropy kernel and — across shards — the drain kernel in SCHED_VIEWS_*), plus what the host knows (views_host: every
+// kernels, the anti-entropy kernel and — across shards — the drain kernel in SCHED_VIEWS_*), plus what the host knows (views_host: every
 // subject that has ever been down — only those are probed, suspected and run timers; all views when the tick carries a host operation or a
-// reaper round).  While exactly ONE subject has ever been down (sv_slot) the host launches BOTH kernels — the single-view one with a
-// parameter block whose planes start at that view and whose subject / down flag are that view's — each looks at the set and one of them
-// returns at once.  SV_CHECK (SERFSIM_SV=2) runs the
-// general kernel alone and raises error 4 if a view outside a one-element set turns out to have business (the set must be a superset).
-constexpr u32 SV_OFF = 0, SV_GENERAL = 1, SV_SINGLE = 2, SV_CHECK = 3;
+// reaper round).
+// Unsharded production ticks without a host operation or a reaper round run as R passes (SV_PASS): the single-slot kernel once per view in
+// ascending slot order, each with a parameter block whose planes start at its view (sv_slot) and whose subject / down flag are that view's.
+// A pass whose view is not in the set skips the node work.  The clock and SerfState travel from pass to pass through the node word, as they
+// do from view to view in the view loop; what the loop keeps in registers travels through the carry plane (CARRY_*).  The first pass
+// evaluates the convergence gate, writes the idle row and decides once which tiles are processed (the decision stays in hot_rd for the later
+// passes; the last one clears it); the last pass takes the tickets and decides whether the cluster can sleep.
+// Sharded runs: while exactly ONE subject has ever been down (sv_slot) the host launches BOTH kernels — the general one and the single-view
+// one for that view — each looks at the set and one of them returns at once.  SV_CHECK (SERFSIM_SV=2) runs the general kernel alone and
+// raises error 4 if a view outside the set turns out to have business (the set must be a superset) — in every tick that would run as passes.
+constexpr u32 SV_OFF = 0, SV_GENERAL = 1, SV_SINGLE = 2, SV_CHECK = 3, SV_PASS = 4;
+// Carry word of a node, valid in tick t iff its tag (bits 8..31) is (t + 1) mod 2^24 (the host runs passes only below tick 2^24 - 1, and
+// the plane is cleared at reset): packets already counted (min(#peers, largest budget) so far), the node stays awake, its timers were due
+// at the start of the tick (its earlier pass rewrote busy bit 3 / node_due exactly), an earlier pass visited it.
+constexpr u32 CARRY_PK = 0xfu, CARRY_AWAKE = 0x10u, CARRY_TDUE = 0x20u, CARRY_SEEN = 0x40u, CARRY_TICKS = 1u << 24;
 constexpr u32 NO_DEADLINE = 0xffffffffu;
 // A tick is skipped (grid-uniform decision of its first instruction) when the last executed tick proved that nothing can happen
 // before SCHED_IDLE_UNTIL and the host scheduled no operation for it.
@@ -195,6 +206,7 @@ struct DrainParams {
 
 void launch_tick(const TickParams& p, bool trace, int grid, cudaStream_t st);
 void launch_tick_single_view(const TickParams& p, int grid, cudaStream_t st);
+void launch_tick_pass(const TickParams& p, int grid, cudaStream_t st);
 void launch_fill_idle_rows(u64* rows, u64* grow_rows, u32 n, const u32* sched, bool trace, cudaStream_t st);
 void launch_pushpull(const TickParams& p, const uint4* snap_rec, const u64* snap_node, bool trace, cudaStream_t st);
 void launch_drain(const DrainParams& p, cudaStream_t st);
