@@ -315,6 +315,48 @@ int serfsim_wire_local_state_batch(serfsim_t* h, uint8_t* out, size_t cap, uint6
 int serfsim_wire_decode_batch(serfsim_t* h, const uint8_t* buf, const uint64_t* offsets, uint32_t n, uint32_t cap,
                               uint64_t* ltime, uint64_t* ids, uint64_t* status_ltimes, uint32_t* n_status);
 
+/* ---- user events on the wire: UserEventMessage (`types/user_event/message.rs`, message type 4), UserEvents / UserEvent
+ *      (`types/user_event/user_events.rs`, `types/user_event.rs`) and the `events` field of PushPull (`types/push_pull.rs:455-587`,
+ *      one entry per occupied ring slot, in ring-index order).  Decoders return pointers INTO the caller's buffer (no copy);
+ *      an empty name or payload decodes as (NULL, 0). ------------------------------------------------------------------------- */
+#define SERFSIM_WIRE_USER_EVENT 4u  /* `types/message.rs:20` */
+typedef struct {                                     /* UserEventMessage */
+  uint64_t ltime;
+  const uint8_t* name; size_t name_len;              /* the event name (UTF-8 on a real node; not checked here) */
+  const uint8_t* payload; size_t payload_len;
+  uint32_t cc, pad;                                  /* "can coalesce" */
+} serfsim_wire_user_event_t;
+typedef struct { const uint8_t* name; size_t name_len; const uint8_t* payload; size_t payload_len; } serfsim_wire_event_t;   /* UserEvent */
+typedef struct { uint64_t ltime; uint32_t n_events, pad; serfsim_wire_event_t* events; } serfsim_wire_user_events_t;         /* UserEvents: one ring slot */
+int serfsim_wire_encode_user_event(const serfsim_wire_user_event_t* m, uint8_t* buf, size_t cap, size_t* len);   /* with the envelope; *len = needed size even on failure */
+int serfsim_wire_decode_user_event(const uint8_t* buf, size_t len, serfsim_wire_user_event_t* out);
+/* PushPull with its ring.  Encode: m as serfsim_wire_encode_push_pull, plus n_ring ring entries written between event_ltime and
+ * query_ltime.  Decode: *n_ring / *n_events are in: the capacities of `ring` and of the event pool `events`, out: the entries
+ * used (SERFSIM_E_INVAL on a shortfall); ring[k].events points into `events`; out->n_events_skipped is 0. */
+int serfsim_wire_encode_push_pull_events(const serfsim_wire_push_pull_t* m, const serfsim_wire_user_events_t* ring, uint32_t n_ring,
+                                         uint8_t* buf, size_t cap, size_t* len);
+int serfsim_wire_decode_push_pull_events(const uint8_t* buf, size_t len, serfsim_wire_push_pull_t* out, serfsim_wire_user_events_t* ring,
+                                         uint32_t* n_ring, serfsim_wire_event_t* events, uint32_t* n_events);
+/* The bytes of the tracked user events (the simulator itself knows only content ids): name and payload of event e, as a real
+ * node's Serf::user_event(name, payload, cc) would carry them.  Call after serfsim_set_user_events with the same n; the table
+ * is kept across serfsim_reset and dropped by the next serfsim_set_user_events.  Rejected (SERFSIM_E_INVAL) when name + payload
+ * exceeds max_user_event_size (512, `options.rs:528`), when the encoded UserEventMessage with its envelope would exceed 512
+ * bytes (`serf/api.rs:251-282`; checked with a 5-byte Lamport time, the widest the device stamps, and cc = false), or when
+ * two events have equal content ids but different bytes or different ids but equal bytes.  Once set, every push-pull message
+ * of serfsim_wire_local_state_batch / _range carries the node's event ring; without it the output is as before. */
+int serfsim_set_user_event_content(serfsim_t* h, uint32_t n, const uint8_t* const* names, const size_t* name_lens,
+                                   const uint8_t* const* payloads, const size_t* payload_lens);
+/* serfsim_wire_local_state_batch over the shard-local nodes [first, first + count): message i (node first + i) occupies
+ * out[offsets[i] .. offsets[i + 1]), offsets[0] = 0.  The whole-shard batch is this range over every local node, byte for
+ * byte.  A node's message can reach a few KB with a content table, so large shards are encoded in chunks. */
+int serfsim_wire_local_state_range(serfsim_t* h, uint32_t first, uint32_t count, uint8_t* out, size_t cap, uint64_t* offsets, size_t* total);
+/* The rings of n concatenated push-pull messages back to the simulator's form, on the device: per message its event clock
+ * (event_ltime), the mask of tracked events its ring holds (bit e: a UserEvent with e's name and payload in an entry whose
+ * ltime is e's Lamport time; tracked events with equal content and ltime resolve to the lowest index) and the number of
+ * events that match no tracked event.  Needs a content table.  A malformed message fails the call (index in the error text). */
+int serfsim_wire_decode_events_batch(serfsim_t* h, const uint8_t* buf, const uint64_t* offsets, uint32_t n,
+                                     uint64_t* event_ltime, uint32_t* seen, uint32_t* n_unmatched);
+
 #ifdef __cplusplus
 }
 #endif

@@ -117,6 +117,27 @@ class Serf {
   std::vector<uint8_t> user_event_seen(uint32_t event) const { std::vector<uint8_t> v(n_); check(serfsim_user_event_seen(h_, event, v.data())); return v; }
   std::vector<LamportTime> event_time() const { std::vector<LamportTime> v(n_); check(serfsim_event_time(h_, v.data())); return v; }
   serfsim_uevent_stats_t user_event_stats() const { serfsim_uevent_stats_t s; check(serfsim_user_event_stats(h_, &s)); return s; }
+  // the (name, payload) bytes of every tracked event, after track_user_events: push-pull messages then carry the event ring
+  void user_event_content(const std::vector<std::string>& names, const std::vector<std::string>& payloads) {
+    if (names.size() != payloads.size()) throw Error(SERFSIM_E_INVAL, "one name and one payload per tracked event");
+    std::vector<const uint8_t*> np, pp;
+    std::vector<size_t> nl, pl;
+    for (size_t e = 0; e < names.size(); ++e) {
+      np.push_back((const uint8_t*)names[e].data()); nl.push_back(names[e].size());
+      pp.push_back((const uint8_t*)payloads[e].data()); pl.push_back(payloads[e].size());
+    }
+    check(serfsim_set_user_event_content(h_, (uint32_t)names.size(), np.data(), nl.data(), pp.data(), pl.data()));
+  }
+  // SerfDelegate::local_state (serf/delegate.rs:386-425) of nodes [first, first + count): the bytes and count + 1 offsets
+  std::pair<std::vector<uint8_t>, std::vector<uint64_t>> local_state(uint32_t first, uint32_t count) const {
+    std::vector<uint64_t> off((size_t)count + 1);
+    size_t total = 0;
+    serfsim_wire_local_state_range(h_, first, count, nullptr, 0, off.data(), &total);      // sizing call
+    std::vector<uint8_t> bytes(total ? total : 1);
+    check(serfsim_wire_local_state_range(h_, first, count, bytes.data(), bytes.size(), off.data(), &total));
+    bytes.resize(total);
+    return {std::move(bytes), std::move(off)};
+  }
 
   // the hot path
   void step(uint32_t ticks = 1) { check(serfsim_step(h_, ticks)); }

@@ -17,6 +17,7 @@
 
 #include "../../include/serfsim.h"
 #include "tick_kernel.cuh"
+#include "wire.cuh"
 
 using namespace sfs;
 
@@ -114,6 +115,8 @@ struct serfsim {
   uint4* d_ue_state = nullptr;     // [stride] 16-byte event records
   u32* d_ue_inbox[2] = {nullptr, nullptr};   // [stride] arrived-event masks per tick parity
   u32* d_ue_ltime = nullptr;       // [MAX_UEVENTS]
+  wire::UeWire ue_wire{};          // wire form of the tracked events (serfsim_set_user_event_content); n = 0: none
+  u8* d_ue_entries = nullptr;      // its UserEvents.events entries on the device
   u64* d_ue_totals = nullptr;      // [8]
   u32 ue_injected = 0;             // tracked events already scheduled (each may be injected once)
   uint4* d_ue_snap = nullptr;      // push-pull rounds: snapshot of the event records (partners read it)
@@ -609,6 +612,7 @@ void free_all(serfsim* h) {
   cudaFree(h->d_subj); cudaFree(h->d_scratch); cudaFree(h->d_stage);
   cudaFree(h->d_byz_ids); cudaFree(h->d_anomaly); cudaFree(h->d_byz_totals); cudaFree(h->d_peer_anomaly);
   cudaFree(h->d_ue_snap); cudaFree(h->d_peer_ue_snap);
+  cudaFree(h->d_ue_entries);
   cudaFree(h->d_ue_state); cudaFree(h->d_ue_inbox[0]); cudaFree(h->d_ue_inbox[1]); cudaFree(h->d_ue_ltime); cudaFree(h->d_ue_totals);
   for (int par = 0; par < 2; ++par) { cudaFree(h->d_win_data[par]); cudaFree(h->d_peer_data[par]); }
   cudaFree(h->d_ctrl); cudaFree(h->d_send_count); cudaFree(h->d_peer_ctrl);
@@ -635,11 +639,12 @@ int getter(serfsim* h, u32 slot, int what, void* out, size_t elem) {
 
 // hooks for wire_codec.cu (the other translation unit behind the C ABI)
 namespace sfs {
-struct WireView { const uint4* rec; const u32* qword; const u64* node_state; const uint4* ue_state; const u32* subj; u32 n_local, stride, R; cudaStream_t stream; };
+struct WireView { const uint4* rec; const u32* qword; const u64* node_state; const uint4* ue_state; const u32* subj; u32 n_local, stride, R; cudaStream_t stream; wire::UeWire ue; };
 int serfsim_fail(int code, const char* msg) { return fail(code, msg); }
 int serfsim_wire_view(const serfsim* h, WireView* out) {
   if (!h) return fail(SERFSIM_E_INVAL, "null handle");
-  *out = WireView{h->d_rec, h->d_qword, h->d_node, h->ue_table.n ? h->d_ue_state : nullptr, h->d_subj, h->count, h->stride, h->R, h->stream};
+  *out = WireView{h->d_rec, h->d_qword, h->d_node, h->ue_table.n ? h->d_ue_state : nullptr, h->d_subj, h->count, h->stride, h->R, h->stream, h->ue_wire};
+  out->ue.ltime = h->d_ue_ltime;
   return 0;
 }
 }  // namespace sfs
@@ -1217,10 +1222,61 @@ int serfsim_set_user_events(serfsim_t* h, uint32_t n_events, const uint32_t* con
   }
   h->ue_table = UeTable{};
   h->ue_table.n = n_events;
+  h->ue_wire.n = 0;                               // a new event table drops the content of the old one
   for (u32 e = 0; e < n_events; ++e) h->ue_table.content[e] = content_ids[e];
   int rc = ue_reset(h);
   if (rc) return rc;
   CU(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// The bytes of the tracked events, encoded once into their UserEvents.events entries (wire.cuh) for the batch encoder.
+int serfsim_set_user_event_content(serfsim_t* h, uint32_t n, const uint8_t* const* names, const size_t* name_lens, const uint8_t* const* payloads,
+                                   const size_t* payload_lens) {
+  if (!h) return fail(SERFSIM_E_INVAL, "null handle");
+  if (!n || n != h->ue_table.n) return fail(SERFSIM_E_INVAL, "serfsim_set_user_event_content: n must equal the n_events of serfsim_set_user_events (> 0)");
+  if (!names || !name_lens || !payloads || !payload_lens) return fail(SERFSIM_E_INVAL, "null argument");
+  for (u32 e = 0; e < n; ++e) {
+    if ((name_lens[e] && !names[e]) || (payload_lens[e] && !payloads[e])) return fail(SERFSIM_E_INVAL, "null argument");
+    // Serf::user_event (serf/api.rs:251-282): name + payload within max_user_event_size, then the encoded message with its
+    // envelope as well — at the widest Lamport time the device can stamp (5 varint bytes) and cc = false
+    if (name_lens[e] > wire::MAX_USER_EVENT_SIZE || payload_lens[e] > wire::MAX_USER_EVENT_SIZE || name_lens[e] + payload_lens[e] > wire::MAX_USER_EVENT_SIZE)
+      return fail(SERFSIM_E_INVAL, "user event " + std::to_string(e) + ": name + payload exceed max_user_event_size (512)");
+    if (wire::envelope_len(wire::uem_payload_len(0xffffffffull, (u32)name_lens[e], (u32)payload_lens[e], false)) > wire::MAX_USER_EVENT_SIZE)
+      return fail(SERFSIM_E_INVAL, "user event " + std::to_string(e) + ": the encoded UserEventMessage exceeds max_user_event_size (512)");
+  }
+  auto bytes_eq = [&](u32 a, u32 b) {
+    return name_lens[a] == name_lens[b] && payload_lens[a] == payload_lens[b] && (!name_lens[a] || !memcmp(names[a], names[b], name_lens[a])) &&
+           (!payload_lens[a] || !memcmp(payloads[a], payloads[b], payload_lens[a]));
+  };
+  for (u32 a = 0; a < n; ++a)
+    for (u32 b = a + 1; b < n; ++b) {
+      const bool same_id = h->ue_table.content[a] == h->ue_table.content[b], same_bytes = bytes_eq(a, b);
+      if (same_id != same_bytes)                     // the device de-duplicates by id, a real node by bytes: they must agree
+        return fail(SERFSIM_E_INVAL, "user events " + std::to_string(a) + " and " + std::to_string(b) +
+                                     (same_id ? ": equal content ids but different bytes" : ": different content ids but equal bytes"));
+    }
+  wire::UeWire t{};
+  std::vector<u8> buf;
+  for (u32 e = 0; e < n; ++e) {
+    const u32 nl = (u32)name_lens[e], pl = (u32)payload_lens[e];
+    t.off[e] = (u32)buf.size();
+    buf.resize(buf.size() + wire::ues_event_entry_len(nl, pl));
+    u8* p = buf.data() + t.off[e];
+    u32 o = 0;
+    p[o++] = wire::UES_EVENT; o += wire::varint_put(p + o, wire::user_event_len(nl, pl));
+    t.bytes[e].name_off = t.off[e] + o + (nl ? 1 + wire::varint_len(nl) : 0); t.bytes[e].name_len = nl;
+    t.bytes[e].pay_off = t.off[e] + o + (nl ? wire::len_delim_len(nl) : 0) + (pl ? 1 + wire::varint_len(pl) : 0); t.bytes[e].pay_len = pl;
+    o += wire::put_user_event(p + o, names[e], nl, payloads[e], pl);
+    if (o != wire::ues_event_entry_len(nl, pl)) return fail(SERFSIM_E_INVAL, "wire: internal length mismatch");
+  }
+  t.off[n] = (u32)buf.size();
+  t.n = n;
+  if (!h->d_ue_entries) CU(cudaMalloc(&h->d_ue_entries, wire::UE_TABLE_MAX * wire::UE_ENTRY_MAX));
+  CU(cudaStreamSynchronize(h->stream));             // no wire kernel is still reading the old table
+  CU(cudaMemcpy(h->d_ue_entries, buf.data(), buf.size(), cudaMemcpyHostToDevice));
+  t.entries = h->d_ue_entries;
+  h->ue_wire = t;
   return 0;
 }
 

@@ -148,6 +148,9 @@ PRODUCT_ONLY = {
     "serfsim_comm_connect": (C.c_int, [_vp, _vp]),
     "serfsim_comm_set_hooks": (C.c_int, [_vp, BARRIER_FN, ALLREDUCE_FN, _vp]),
     "serfsim_comm_loopback": (C.c_int, [_vp]),
+    "serfsim_set_user_event_content": (C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
+    "serfsim_wire_local_state_range": (C.c_int, [_vp, _u32, _u32, _vp, C.c_size_t, _vp, C.POINTER(C.c_size_t)]),
+    "serfsim_wire_decode_events_batch": (C.c_int, [_vp, _vp, _vp, _u32, _vp, _vp, _vp]),
 }
 
 _LIB = None
@@ -339,6 +342,42 @@ class GossipSim:
         t = _u64()
         self._check(self._fn("user_event_ltime")(self._h, int(event), C.byref(t)))
         return t.value
+
+    def set_user_event_content(self, names, payloads):
+        """The bytes of every tracked user event — what Serf::user_event(name, payload, cc) carries — after set_user_events with
+        as many events.  From then on every push-pull message (wire_local_state_range) carries the node's event ring."""
+        if len(names) != len(payloads):
+            raise ValueError("one name and one payload per tracked event")
+        raw = [x.encode() if isinstance(x, str) else bytes(x) for x in list(names) + list(payloads)]
+        bufs = [C.create_string_buffer(b, max(1, len(b))) for b in raw]
+        n = len(names)
+        ptrs = [C.addressof(b) for b in bufs]
+        lens = [len(b) for b in raw]
+        self._check(self._lib.serfsim_set_user_event_content(self._h, n, (_vp * n)(*ptrs[:n]), (C.c_size_t * n)(*lens[:n]),
+                                                             (_vp * n)(*ptrs[n:]), (C.c_size_t * n)(*lens[n:])))
+
+    def wire_local_state_range(self, first=0, count=None):
+        """SerfDelegate::local_state of the shard-local nodes [first, first + count), encoded on the device:
+        (uint8 bytes, uint64 offsets[count + 1]); message i is bytes[offsets[i]:offsets[i + 1]]."""
+        count = self.count - first if count is None else count
+        off = np.zeros(count + 1, np.uint64)
+        tot = C.c_size_t()
+        f = self._lib.serfsim_wire_local_state_range
+        f(self._h, first, count, None, 0, off.ctypes.data, C.byref(tot))                 # sizing call: reports the total
+        out = np.empty(max(1, tot.value), np.uint8)
+        self._check(f(self._h, first, count, out.ctypes.data, out.size, off.ctypes.data, C.byref(tot)))
+        return out[:tot.value], off
+
+    def wire_decode_events(self, buf, offsets):
+        """The event rings of n push-pull messages back to the simulator's form, on the device: (event_ltime uint64[n],
+        seen uint32[n] — bit e: tracked event e is in the ring —, unmatched uint32[n] — events matching no tracked event)."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = offsets.size - 1
+        ev, seen, um = np.zeros(n, np.uint64), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
+        self._check(self._lib.serfsim_wire_decode_events_batch(self._h, buf.ctypes.data, offsets.ctypes.data, n, ev.ctypes.data,
+                                                               seen.ctypes.data, um.ctypes.data))
+        return ev, seen, um
 
     def user_event_stats(self):
         s = UserEventStats()
