@@ -184,6 +184,7 @@ struct serfsim {
   bool l2_window = false;           // SERFSIM_L2_WINDOW=1: stream access-policy window over the inbox being written
   bool no_skip = false;             // SERFSIM_NO_SKIP=1: process every tile every tick (A/B measurements)
   bool compact = true;              // SERFSIM_COMPACT=0: tile-by-tile walk in unsaturated ticks too (A/B measurements)
+  bool dedup = true;                // SERFSIM_DEDUP=0: unsharded sends issue every RED, also those that change nothing (A/B measurements)
   // asynchronous result read-back (serfsim_results_async): extraction into a ring of staging buffers on the launch stream,
   // device→host copies on a second stream so that they overlap the ticks of the caller's next step
   struct ResBuf { unsigned char* d = nullptr; cudaEvent_t copied = nullptr; bool used = false; };
@@ -295,6 +296,7 @@ int launch_ticks(serfsim* h, u32 n) {
     p.stride = h->stride; p.n_tiles = h->n_tiles; p.tiles_per_cta = (h->n_tiles + h->grid - 1) / h->grid;
     p.force_all = (h->cfg.trace != 0) || h->no_skip || p.reap_now;
     p.compact = h->compact ? 1u : 0u;
+    p.dedup = h->dedup ? 1u : 0u;
     p.udeg = h->udeg; p.ahead = h->ahead;
     p.tile_due = h->d_tile_due; p.node_due = h->d_node_due; p.hot_static = h->d_hot_static; p.sched = h->d_sched;
     p.sleep_on = (h->no_skip || h->byz_on) ? 0u : 1u;          // injectors send every tick: the cluster never sleeps
@@ -765,6 +767,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   }
   if (const char* e = getenv("SERFSIM_NO_SKIP")) h->no_skip = atoi(e) != 0;
   if (const char* e = getenv("SERFSIM_COMPACT")) h->compact = atoi(e) != 0;
+  if (const char* e = getenv("SERFSIM_DEDUP")) h->dedup = atoi(e) != 0;
   if (const char* e = getenv("SERFSIM_AHEAD")) h->ahead = (u32)std::min(2, std::max(0, atoi(e)));
   if (const char* e = getenv("SERFSIM_SV")) h->sv = (u32)std::min(2, std::max(0, atoi(e)));
   if (cfg->world_size > 1) {

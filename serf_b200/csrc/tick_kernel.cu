@@ -88,6 +88,9 @@ __device__ __forceinline__ void st_u64_stream(u64* ptr, u64 v, u64 pol) {
 __device__ __forceinline__ void red_max_resident(u32* ptr, u32 v, u64 pol) {   // RED.MAX, result unused, line kept in L2
   asm volatile("red.relaxed.gpu.global.max.L2::cache_hint.u32 [%0], %1, %2;" :: "l"(ptr), "r"(v), "l"(pol) : "memory");
 }
+__device__ __forceinline__ u32 peek_inbox(const u32* ptr, u64 pol) {   // a word of the plane being reduced into (any value it held during the launch)
+  u32 v; asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(ptr), "l"(pol)); return v;
+}
 __device__ __forceinline__ void st_release_sys(u32* ptr, u32 v) { asm volatile("st.release.sys.global.u32 [%0], %1;" :: "l"(ptr), "r"(v) : "memory"); }
 __device__ __forceinline__ u32 ld_acquire_sys(const u32* ptr) { u32 f; asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(f) : "l"(ptr) : "memory"); return f; }
 #else   // SERFSIM_EMU: the same accessors as plain C++ (tests/emu compiles this file for the host; cache hints have no meaning there)
@@ -102,6 +105,7 @@ inline u32 ld_u32_stream(const u32* ptr, u64) { emu::probes[11] += 4; return *pt
 inline void st_u32_stream(u32* ptr, u32 v, u64) { emu::probes[12] += 4; *ptr = v; }
 inline void st_u64_stream(u64* ptr, u64 v, u64) { emu::probes[13] += 8; *ptr = v; }
 inline void red_max_resident(u32* ptr, u32 v, u64) { emu::probes[14] += 4; if (v > *ptr) *ptr = v; }
+inline u32 peek_inbox(const u32* ptr, u64) { emu::probes[11] += 4; return *ptr; }
 inline void st_release_sys(u32* ptr, u32 v) { __atomic_store_n(ptr, v, __ATOMIC_RELEASE); }     // peers are other threads of the test process
 inline u32 ld_acquire_sys(const u32* ptr) {                 // polled in a loop by the drain kernel: be polite to the peer threads, and never hang a test run
   static thread_local const u32* last = nullptr;
@@ -185,11 +189,15 @@ __device__ __forceinline__ u32 shard_of(const TickParams& p, u32 dst, u32& dloc)
   return q;
 }
 
+// held: what the sender read from the destination word earlier in this launch (0: nothing read).  The words of the plane only
+// grow during a launch (RED.MAX is the only write to the planes a launch sends into), so held ≥ val1 means the word already is,
+// and will stay, at least val1: the RED would change nothing and is not issued.  The tile is marked all the same.
 template <bool SHARDED>
-__device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* plane, u32 dst, u32 kind, u32 s, u32 val1, u64 pol_last, bool mark) {
+__device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* plane, u32 dst, u32 kind, u32 s, u32 val1, u64 pol_last, bool mark, u32 held = 0) {
   const u32 dl = dst - p.first;
   if (!SHARDED || dl < p.n_local) {
-    red_max_resident(plane + dl, val1, pol_last);
+    if (val1 > held) red_max_resident(plane + dl, val1, pol_last);
+    else SFS_PROBE(22);
     if (mark) p.hot_wr[dl >> TILE_SHIFT] = 1;  // sparse ticks only: tell the next tick which tiles received something
   } else {
     u32 dloc;
@@ -216,6 +224,20 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
       else *p.overflow = 2;
     }
   }
+}
+
+// Unsharded sends of one entry to its first n targets.  With p.dedup (SERFSIM_DEDUP, on by default):  In a saturated tick every sender of a wave
+// sends the same value for a (kind, view), and a destination gets about Poisson(fanout) copies: most REDs would write a value the
+// word already holds.  The destination words are read first, all together (one round trip per entry, not per target), and only
+// the REDs that can raise a word are issued.  Exact whatever the reads return (see deliver).
+template <int FMAX>
+__device__ __forceinline__ void send_deduped(const TickParams& p, u32* plane, const u32 (&tg)[FMAX], u32 n, u32 val1, u64 pol_last, bool mark) {
+  u32 held[FMAX];
+#pragma unroll
+  for (int k = 0; k < FMAX; ++k) held[k] = ((u32)k < n && p.dedup) ? peek_inbox(plane + (tg[k] - p.first), pol_last) : 0u;
+#pragma unroll
+  for (int k = 0; k < FMAX; ++k)
+    if ((u32)k < n) deliver<false>(p, nullptr, plane, tg[k], 0, 0, val1, pol_last, mark, held[k]);
 }
 
 // Copy the warp's staged entries into the peers' windows (whole warp, convergent) in runs of whole 32-entry blocks (256+
@@ -663,11 +685,17 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
         u32* const planeM = p.inbox_wr + (size_t)(KIND_ML * R + s) * nl;
         const u32 vL = leave_key(r.qleave, (r.flags & FLAG_QPRUNE) != 0) + 1, vJ = r.qjoin + 1, vM = ml_key(r) + 1;
         const u32 sL = min(r.txl, nt), sJ = min(r.txj, nt), sM = min(r.txm, nt);     // entry e goes to targets 0 .. min(tx_e, nt)-1
+        if (!SHARDED) {
+          send_deduped<FMAX>(p, planeL, tg, sL, vL, pol_last, mark);
+          send_deduped<FMAX>(p, planeJ, tg, sJ, vJ, pol_last, mark);
+          send_deduped<FMAX>(p, planeM, tg, sM, vM, pol_last, mark);
+        } else {
 #pragma unroll
-        for (int k = 0; k < FMAX; ++k) {
-          if ((u32)k < sL) deliver<SHARDED>(p, xs, planeL, tg[k], KIND_LEAVE, s, vL, pol_last, mark);
-          if ((u32)k < sJ) deliver<SHARDED>(p, xs, planeJ, tg[k], KIND_JOIN, s, vJ, pol_last, mark);
-          if ((u32)k < sM) deliver<SHARDED>(p, xs, planeM, tg[k], KIND_ML, s, vM, pol_last, mark);
+          for (int k = 0; k < FMAX; ++k) {
+            if ((u32)k < sL) deliver<SHARDED>(p, xs, planeL, tg[k], KIND_LEAVE, s, vL, pol_last, mark);
+            if ((u32)k < sJ) deliver<SHARDED>(p, xs, planeJ, tg[k], KIND_JOIN, s, vJ, pol_last, mark);
+            if ((u32)k < sM) deliver<SHARDED>(p, xs, planeM, tg[k], KIND_ML, s, vM, pol_last, mark);
+          }
         }
         if (R1) { c.kLJ += sL | (sJ << 16); c.kM += sM; c.pe += min(mx, nt) << 16; }
         else { c.kL += sL; c.kJ += sJ; c.kM += sM; c.edges += min(mx, nt); }
