@@ -86,13 +86,17 @@ typedef struct serfsim_config {
   uint32_t n_nodes;                   /* N virtual members, dense ids 0..N-1                         */
   uint32_t slots;                     /* R tracked subjects; every node holds a view of each (1..16) */
   uint32_t fanout;                    /* memberlist gossip_nodes (1..8), LAN default 3               */
-  uint32_t retransmit_mult;           /* memberlist retransmit_mult, LAN default 4                   */
-  uint32_t suspicion_mult;            /* LAN default 4                                               */
+  uint32_t retransmit_mult;           /* memberlist retransmit_mult, LAN default 4; the limit retransmit_mult x
+                                         ceil(log10(n_nodes + 1)), in 64 bits, must be 1..255       */
+  uint32_t suspicion_mult;            /* LAN default 4; 0..9 (k = suspicion_mult - 2 <= 7 confirmations) */
   uint32_t suspicion_max_timeout_mult;/* LAN default 6                                               */
   uint32_t probe_interval_ticks;      /* probe_interval / gossip_interval (LAN 1 s / 200 ms = 5); 0 = no probing */
-  uint32_t gossip_interval_ms;        /* wall-clock length of one tick (LAN 200); only scales the suspicion table */
-  uint32_t init_status_ltime;         /* bootstrap MemberState.status_time of every view (default 1) */
-  uint32_t init_clock;                /* bootstrap LamportClock of every node (default 2)            */
+  uint32_t gossip_interval_ms;        /* wall-clock length of one tick (LAN 200); only scales the suspicion table.
+                                         The suspicion timeouts' ms arithmetic must fit in int64 and every timeout
+                                         must be at most 2^30 ticks (DESIGN.md §2 rule 10)            */
+  uint32_t init_status_ltime;         /* bootstrap MemberState.status_time of every view (default 1); < 0x7FFFFFE0 */
+  uint32_t init_clock;                /* bootstrap LamportClock of every node (default 2); < 0x7FFFFFE0
+                                         (16 below the device's Lamport limit 0x7FFFFFF0)            */
   uint32_t trace;                     /* 1: fill the per-tick state hash (parity runs); 0: skip it   */
   uint64_t seed;                      /* keys the counter RNG (Philox4x32-10)                        */
   int32_t  device;                    /* CUDA ordinal (-1 = current)                                 */

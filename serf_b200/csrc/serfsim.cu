@@ -36,12 +36,43 @@ int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
 struct HostOp { u32 tick, op, node, slot; u64 seq; };
 
-// memberlist retransmit limit: retransmit_mult * ceil(log10(n + 1))  [external crate, restated]
-u32 retransmit_limit(u32 mult, u64 n) {
-  u32 digits = 0;
+// memberlist retransmit limit: retransmit_mult * ceil(log10(n + 1))  [external crate, restated].  In 64 bits: serfsim_create
+// rejects a product outside 1..255 (the budgets are u8) instead of letting it wrap in u32.
+u64 retransmit_limit(u32 mult, u64 n) {
+  u64 digits = 0;
   u64 p = 1;
   while (p < n + 1) { p *= 10; ++digits; }
-  return mult * digits;
+  return (u64)mult * digits;
+}
+
+// Bounds of the configuration's numeric range (serfsim.h, DESIGN §2 rule 10).
+//  - Suspicion timeouts: at most 2^30 ticks.  A run stores a 64-byte trace row per tick, so no device holds 2^31 ticks of one
+//    run; tick + timeout and the confirmation update deadline - timeout[c] + timeout[c+1] then stay below 2^31 + 2^30, inside u32
+//    and never 0 ("no timer").  2^30 ticks are 6.8 years at 200 ms per tick.
+//  - Bootstrap Lamport times (init_clock, init_status_ltime): below LTIME_LIMIT - 16, so the bootstrap state is representable
+//    and a run starts at least 16 Lamport increments away from SERFSIM_E_OVERFLOW.
+constexpr u64 TIMEOUT_LIMIT_TICKS = 1ull << 30;
+constexpr u32 INIT_LTIME_BOUND = LTIME_LIMIT - 16;
+
+const char* const kTimeoutTooLong =
+    "suspicion timeout longer than 2^30 ticks (suspicion_mult, suspicion_max_timeout_mult, probe_interval_ticks, gossip_interval_ms)";
+
+// The integer (ms) part of suspicion_table in exact 128-bit arithmetic: null when every intermediate fits in int64 and the
+// exact timeouts are at most TIMEOUT_LIMIT_TICKS, else the reason.  The entries lie between ceil(min_ms / tick_ms) and
+// ceil(max(min_ms, max_ms) / tick_ms) (just the former when k < 1), so that bounds them all (up to the rounding of the double step,
+// which serfsim_create checks on the table itself).  Only a config that passes this is given to suspicion_table.
+const char* suspicion_table_unrepresentable(u32 susp_mult, u32 max_mult, u32 probe_ticks, u32 tick_ms, u64 n) {
+  const double node_scale = std::max(1.0, std::log10(std::max(1.0, (double)n)));
+  const __int128 i64max = (__int128)INT64_MAX;
+  const __int128 interval_ms = (__int128)probe_ticks * tick_ms;
+  const __int128 prod = (__int128)susp_mult * (int64_t)(node_scale * 1000.0) * interval_ms;
+  if (interval_ms > i64max || prod > i64max) return "suspicion timeout: suspicion_mult x probe_interval_ticks x gossip_interval_ms overflows the 64-bit ms arithmetic";
+  const __int128 min_ms = prod / 1000, max_ms = (__int128)max_mult * min_ms;
+  if (max_ms > i64max) return "suspicion timeout: suspicion_max_timeout_mult x the minimum timeout overflows the 64-bit ms arithmetic";
+  const bool confirmations = (int64_t)susp_mult - 2 >= 1 && (int64_t)n - 2 >= (int64_t)susp_mult - 2;   // k >= 1: max_ms is used
+  const __int128 top = confirmations ? std::max(min_ms, max_ms) : min_ms;
+  if ((top + tick_ms - 1) / tick_ms > (__int128)TIMEOUT_LIMIT_TICKS) return kTimeoutTooLong;
+  return nullptr;
 }
 
 // memberlist suspicion timeouts (Lifeguard), in ticks  [external crate, restated]:
@@ -687,6 +718,17 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   if (cfg->gossip_interval_ms == 0) return fail(SERFSIM_E_INVAL, "gossip_interval_ms must be > 0");
   if (cfg->push_pull_interval_ticks < 0) return fail(SERFSIM_E_INVAL, "push_pull_interval_ticks must be >= 0");
   if (cfg->suspicion_mult >= 2 && cfg->suspicion_mult - 2 > MAX_K) return fail(SERFSIM_E_INVAL, "suspicion_mult too large");
+  if (cfg->init_clock >= INIT_LTIME_BOUND) return fail(SERFSIM_E_INVAL, "init_clock must be below LTIME_LIMIT - 16 (0x7FFFFFE0)");
+  if (cfg->init_status_ltime >= INIT_LTIME_BOUND) return fail(SERFSIM_E_INVAL, "init_status_ltime must be below LTIME_LIMIT - 16 (0x7FFFFFE0)");
+  {
+    const u64 limit = retransmit_limit(cfg->retransmit_mult, cfg->n_nodes);
+    if (limit == 0 || limit > 255) return fail(SERFSIM_E_INVAL, "retransmit limit (retransmit_mult x digits of n_nodes) must be 1..255");
+    const u32 probe = cfg->probe_interval_ticks ? cfg->probe_interval_ticks : 1;
+    const char* why = suspicion_table_unrepresentable(cfg->suspicion_mult, cfg->suspicion_max_timeout_mult, probe, cfg->gossip_interval_ms, cfg->n_nodes);
+    if (why) return fail(SERFSIM_E_INVAL, why);
+    for (u32 t : suspicion_table(cfg->suspicion_mult, cfg->suspicion_max_timeout_mult, probe, cfg->gossip_interval_ms, cfg->n_nodes))
+      if (t > TIMEOUT_LIMIT_TICKS) return fail(SERFSIM_E_INVAL, kTimeoutTooLong);      // the double step rounded past the bound
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(SERFSIM_E_NO_DEVICE, "no CUDA device: serfsim has no CPU execution path");
@@ -704,8 +746,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   h->count = (u32)std::min<u64>(h->shard_size, (u64)h->N - h->first);
   if (h->count == 0) { delete h; return fail(SERFSIM_E_INVAL, "empty shard"); }
   if (h->shard_size >= (1u << 26)) { delete h; return fail(SERFSIM_E_INVAL, "shard larger than 2^26 nodes"); }
-  h->rules.limit = retransmit_limit(cfg->retransmit_mult, h->N);
-  if (h->rules.limit == 0 || h->rules.limit > 255) { delete h; return fail(SERFSIM_E_INVAL, "retransmit limit must be 1..255"); }
+  h->rules.limit = (u32)retransmit_limit(cfg->retransmit_mult, h->N);      // 1..255: checked above
   auto tab = suspicion_table(cfg->suspicion_mult, cfg->suspicion_max_timeout_mult, cfg->probe_interval_ticks ? cfg->probe_interval_ticks : 1, cfg->gossip_interval_ms, h->N);
   h->rules.k = (u32)tab.size() - 1;
   for (size_t i = 0; i < tab.size(); ++i) h->rules.timeout[i] = tab[i];
