@@ -262,6 +262,10 @@ int serfsim_last_step_device_ms(serfsim_t* h, double* ms, uint64_t* kernel_launc
  * step, then read the duration in milliseconds of ticks [first_tick, first_tick + n). */
 int serfsim_set_tick_timing(serfsim_t* h, int enabled);
 int serfsim_tick_times(serfsim_t* h, uint32_t first_tick, uint32_t n, float* ms_out);
+/* Messages (leave, join, memberlist entries) each tracked subject's view sent in ticks [first_tick, first_tick + n), as counted by
+ * the per-view passes of unsharded multi-slot runs; ticks that ran no passes (host operations, reaper rounds, trace mode, single-slot
+ * and sharded runs) read as zero.  out: [n][slots][3]. */
+int serfsim_tick_view_kinds(serfsim_t* h, uint32_t first_tick, uint32_t n, uint32_t* out);
 
 /* ---- multi-GPU (one process per GPU; ids sharded by contiguous range) ---------------- */
 /* Size of the opaque blob a rank publishes to its peers, and the exchange itself: every

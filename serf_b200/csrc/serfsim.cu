@@ -134,6 +134,7 @@ struct serfsim {
   size_t ev_cap = 0;
   u64* d_trace = nullptr;          // [trace_cap][8]
   u32* d_kinds = nullptr;          // [trace_cap+1][4]; row t+1 = messages by kind sent in tick t
+  u32* d_view_kinds = nullptr;     // [trace_cap+1][R][4]; row t+1 = messages by view and kind sent in tick t by per-view passes (zero otherwise)
   u32* d_ones = nullptr;           // [4] non-zero (multi-GPU: never skip an inbox plane)
   u32 trace_cap = 0;
   u32* d_overflow = nullptr;       // device address of pin_overflow (mapped pinned host memory: written by kernels on the rare error paths, read by the host without a copy)
@@ -238,21 +239,24 @@ int ensure_trace(serfsim* h, u32 need) {
   if (need <= h->trace_cap) return 0;
   u32 cap = std::max<u32>(1024, h->trace_cap);
   while (cap < need) cap *= 2;
-  u64* nt = nullptr; u32* nk = nullptr; u64* ng = nullptr;
+  u64* nt = nullptr; u32* nk = nullptr; u32* nv = nullptr; u64* ng = nullptr;
   const bool sharded = h->cfg.world_size > 1;
   CU(cudaMalloc(&nt, (size_t)cap * 8 * sizeof(u64)));
   CU(cudaMalloc(&nk, ((size_t)cap + 1) * 4 * sizeof(u32)));
+  CU(cudaMalloc(&nv, ((size_t)cap + 1) * h->R * 4 * sizeof(u32)));
   CU(cudaMemsetAsync(nt, 0, (size_t)cap * 8 * sizeof(u64), h->stream));
   CU(cudaMemsetAsync(nk, 0, ((size_t)cap + 1) * 4 * sizeof(u32), h->stream));
+  CU(cudaMemsetAsync(nv, 0, ((size_t)cap + 1) * h->R * 4 * sizeof(u32), h->stream));
   if (sharded) { CU(cudaMalloc(&ng, (size_t)cap * 8 * sizeof(u64))); CU(cudaMemsetAsync(ng, 0, (size_t)cap * 8 * sizeof(u64), h->stream)); }
   if (h->d_trace) {
     CU(cudaMemcpyAsync(nt, h->d_trace, (size_t)h->trace_cap * 8 * sizeof(u64), cudaMemcpyDeviceToDevice, h->stream));
     CU(cudaMemcpyAsync(nk, h->d_kinds, ((size_t)h->trace_cap + 1) * 4 * sizeof(u32), cudaMemcpyDeviceToDevice, h->stream));
+    CU(cudaMemcpyAsync(nv, h->d_view_kinds, ((size_t)h->trace_cap + 1) * h->R * 4 * sizeof(u32), cudaMemcpyDeviceToDevice, h->stream));
     if (sharded) CU(cudaMemcpyAsync(ng, h->d_grow, (size_t)h->trace_cap * 8 * sizeof(u64), cudaMemcpyDeviceToDevice, h->stream));
     CU(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_grow);
+    cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds); cudaFree(h->d_grow);
   }
-  h->d_trace = nt; h->d_kinds = nk; h->d_grow = ng; h->trace_cap = cap;
+  h->d_trace = nt; h->d_kinds = nk; h->d_view_kinds = nv; h->d_grow = ng; h->trace_cap = cap;
   return 0;
 }
 
@@ -281,6 +285,28 @@ int upload_ops(serfsim* h) {
 
 bool future_ops(const serfsim* h, u32 after_tick) {       // any op scheduled at tick > after_tick
   return !h->ops.empty() && h->ops.back().tick > after_tick;
+}
+
+bool ops_at(const serfsim* h, u32 t) {
+  auto it = std::lower_bound(h->ops.begin(), h->ops.end(), t, [](const HostOp& o, u32 tt) { return o.tick < tt; });
+  return it != h->ops.end() && it->tick == t;
+}
+bool reap_tick(const serfsim* h, u32 t) { return h->cfg.reap_interval_ticks && ((t + 1) % h->cfg.reap_interval_ticks) == 0; }
+// Multi-slot production runs: does tick t run as per-view passes (SV_PASS, tick_kernel.cuh)?  Unsharded ticks without a host operation
+// or a reaper round.  (mode: the SERFSIM_SV mode it is asked for; check mode takes the same ticks to the general kernel)
+bool pass_tick(const serfsim* h, u32 t, u32 mode) {
+  const bool sleep_on = !h->no_skip && !h->byz_on;
+  return h->sv == mode && h->R > 1 && h->R < 32 && !h->cfg.trace && sleep_on && h->cfg.world_size == 1 && !ops_at(h, t) && !reap_tick(h, t) &&
+         t + 1 < CARRY_TICKS;
+}
+// The passes of tick t + 1 choose their loads from their own views' counters of tick t (TickParams::view_kinds_prev) only if every
+// inbox write of tick t was a pass's: otherwise (general kernel — host operation, reaper round, trace mode, SERFSIM_SV=0/2 — anti-entropy
+// round, injectors, sharded runs) the general kernel's sends and the other writers are not in them, and the passes fall back to the whole
+// tick's counters.  Ticks the host jumped over or the device skipped sent nothing: their zero rows are exact either way.  This is the
+// one place that decides it.
+bool view_kinds_valid(const serfsim* h, u32 t) {
+  const u32 pp = (u32)std::max(0, h->cfg.push_pull_interval_ticks);
+  return pass_tick(h, t, 1) && !(pp && (t + 1) % pp == 0);          // (injectors: pass_tick is false)
 }
 
 // Launch n ticks on the stream (no synchronisation).
@@ -322,7 +348,7 @@ int launch_ticks(serfsim* h, u32 n) {
     p.overflow = h->d_overflow;
     p.hot_rd = h->d_hot[(t & 1) ^ 1]; p.hot_wr = h->d_hot[t & 1];
     p.stage_col_bytes = h->stage_col_bytes;
-    p.reap_now = (h->cfg.reap_interval_ticks && ((t + 1) % h->cfg.reap_interval_ticks) == 0) ? 1u : 0u;
+    p.reap_now = reap_tick(h, t) ? 1u : 0u;
     p.tombstone_ticks = h->cfg.tombstone_timeout_ticks; p.reconnect_ticks = h->cfg.reconnect_timeout_ticks; p.intent_ticks = h->cfg.recent_intent_timeout_ticks;
     p.stride = h->stride; p.n_tiles = h->n_tiles; p.tiles_per_cta = (h->n_tiles + h->grid - 1) / h->grid;
     p.force_all = (h->cfg.trace != 0) || h->no_skip || p.reap_now;
@@ -379,20 +405,23 @@ int launch_ticks(serfsim* h, u32 n) {
     // per-view passes of the single-slot kernel.  Sharded: while exactly one subject has ever been down, the general kernel and the
     // single-view kernel are both launched and the device decides.
     const bool sv_ok = h->sv && h->R > 1 && h->R < 32 && !h->cfg.trace && p.sleep_on && !h->byz_on;
-    const bool pass_tick = sv_ok && !sharded && ee == eb && !p.reap_now && t + 1 < CARRY_TICKS;
+    const bool passes = pass_tick(h, t, 1), check = pass_tick(h, t, 2);
     const bool dual = sv_ok && sharded && __builtin_popcount(h->ever_down) == 1;
-    if (pass_tick || dual) {
+    if (passes || check || dual) {
       const bool all = ee > eb || p.reap_now;                 // a host operation or a reaper round visits every view
       p.views_host = all ? 0xffffffffu : h->ever_down;
       p.sv_mode = h->sv == 2 ? SV_CHECK : SV_GENERAL;
       p.sv_slot = h->ever_down ? (u32)__builtin_ctz(h->ever_down) : 0u; p.sv_R = h->R;
     }
-    if (pass_tick && h->sv == 1) {
+    if (passes) {
       p.sv_mode = SV_PASS; p.carry = h->d_carry;
       p.tiles_per_cta = (h->n_tiles + h->grid_sv - 1) / h->grid_sv;
+      const bool own = t > 0 && view_kinds_valid(h, t - 1);
       for (u32 s0 = 0; s0 < h->R; ++s0) {                  // ascending slot order: what the view loop carries from view to view travels through memory
         TickParams q = p;                                  // the planes as the single-slot kernel sees them: they start at view s0
         q.gate.evaluate = s0 == 0 ? p.gate.evaluate : 0u; q.sv_wshift = s0; q.sv_slot = s0;
+        q.view_kinds_prev = own ? h->d_view_kinds + ((size_t)t * h->R + s0) * 4 : p.kinds_prev;
+        q.view_kinds_cur = h->d_view_kinds + (((size_t)t + 1) * h->R + s0) * 4;
         q.rec = p.rec + 2 * (size_t)s0 * h->stride; q.qword = p.qword + (size_t)s0 * h->stride;
         q.inbox_rd = p.inbox_rd + (size_t)s0 * h->stride; q.inbox_wr = p.inbox_wr + (size_t)s0 * h->stride;
         q.subj[0] = p.subj[s0]; q.down_mask = (p.down_mask >> s0) & 1u;
@@ -622,6 +651,7 @@ int do_reset(serfsim* h, u64 seed) {
   if (h->d_trace) {
     CU(cudaMemsetAsync(h->d_trace, 0, (size_t)h->trace_cap * 8 * sizeof(u64), h->stream));
     CU(cudaMemsetAsync(h->d_kinds, 0, ((size_t)h->trace_cap + 1) * 4 * sizeof(u32), h->stream));
+    CU(cudaMemsetAsync(h->d_view_kinds, 0, ((size_t)h->trace_cap + 1) * h->R * 4 * sizeof(u32), h->stream));
   }
   if (h->d_grow) CU(cudaMemsetAsync(h->d_grow, 0, (size_t)h->trace_cap * 8 * sizeof(u64), h->stream));
   CU(cudaMemsetAsync(h->d_runctl, 0, 2 * sizeof(u32), h->stream));
@@ -640,7 +670,7 @@ void free_all(serfsim* h) {
   cudaFree(h->d_hot[0]); cudaFree(h->d_hot[1]); cudaFree(h->d_busy); cudaFree(h->d_watch); cudaFree(h->d_snap_rec); cudaFree(h->d_snap_node); cudaFree(h->d_peer_snap_rec); cudaFree(h->d_peer_snap_node);
   cudaFree(h->d_qword);
   cudaFree(h->d_rec); cudaFree(h->d_inbox[0]); cudaFree(h->d_inbox[1]); cudaFree(h->d_node); cudaFree(h->d_rowptr); cudaFree(h->d_col);
-  cudaFree(h->d_ev_node); cudaFree(h->d_ev_op); cudaFree(h->d_ev_slot); cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_ones);
+  cudaFree(h->d_ev_node); cudaFree(h->d_ev_op); cudaFree(h->d_ev_slot); cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds); cudaFree(h->d_ones);
   if (h->pin_overflow) cudaFreeHost(h->pin_overflow);
   cudaFree(h->d_subj); cudaFree(h->d_scratch); cudaFree(h->d_stage);
   cudaFree(h->d_byz_ids); cudaFree(h->d_anomaly); cudaFree(h->d_byz_totals); cudaFree(h->d_peer_anomaly);
@@ -1410,6 +1440,17 @@ int serfsim_tick_times(serfsim_t* h, uint32_t first_tick, uint32_t n, float* ms_
   if (((size_t)first_tick + n) * 2 > h->tick_ev.size()) return fail(SERFSIM_E_INVAL, "tick timing was not enabled for that range");
   CU(cudaStreamSynchronize(h->stream));
   for (u32 i = 0; i < n; ++i) CU(cudaEventElapsedTime(ms_out + i, h->tick_ev[2 * ((size_t)first_tick + i)], h->tick_ev[2 * ((size_t)first_tick + i) + 1]));
+  return 0;
+}
+int serfsim_tick_view_kinds(serfsim_t* h, uint32_t first_tick, uint32_t n, uint32_t* out) {
+  if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
+  if ((size_t)first_tick + n > h->tick) return fail(SERFSIM_E_INVAL, "ticks not run yet");
+  if (!n) return 0;
+  std::vector<u32> rows((size_t)n * h->R * 4);
+  CU(cudaMemcpyAsync(rows.data(), h->d_view_kinds + ((size_t)first_tick + 1) * h->R * 4, rows.size() * sizeof(u32), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  for (size_t i = 0; i < (size_t)n * h->R; ++i)
+    for (u32 k = 0; k < 3; ++k) out[i * 3 + k] = rows[i * 4 + k];
   return 0;
 }
 

@@ -406,8 +406,15 @@ __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool k
 // Has the node anything to do this tick?  (due: its tile's earliest suspicion deadline has been reached — then a node that runs timers
 // looks at its OWN earliest deadline: only if that has been reached too does it visit its views; otherwise it hands the deadline back
 // to the timer wheel, sleeping_deadline(), without touching a record.)
+// A pass does not look at the awake bit (busy bit 0): it says that SOME view of the node keeps a queue or a watcher's probe duty.  The
+// pass's own view's queue is in `any` (its queue word), probe duty comes with the static watcher bit 2, and a view with neither, no mail,
+// no host operation and no timer due has nothing to do: the view loop leaves it unvisited too.  So a pass skips the nodes that are
+// awake only for another view's sake (in a tick in which one view's wave keeps nearly every node awake, nearly all of them).
+template <bool PASS = false>
+__device__ __forceinline__ u32 busy_business(u32 busy) { return busy & (PASS ? 6u : 7u); }
+template <bool PASS = false>
 __device__ __forceinline__ bool node_active(const TickParams& p, const Pre& x, bool due) {
-  return (x.busy & 7u) != 0 || x.any != 0 || p.reap_now != 0 || (due && (x.busy & 8u) && x.nd <= p.tick);
+  return busy_business<PASS>(x.busy) != 0 || x.any != 0 || p.reap_now != 0 || (due && (x.busy & 8u) && x.nd <= p.tick);
 }
 
 // Multi-slot runs, saturated ticks: what a node needs beyond its `Pre` words, requested ONE TILE AHEAD together with them — the node
@@ -553,7 +560,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   bool timers_due = sleeping <= p.tick;
   u32 cr = 0;                                            // PASS: what the earlier passes of this tick did at this node
   if (PASS && due) { cr = carry_of(p, vl); if (cr & CARRY_SEEN) timers_due = (cr & CARRY_TDUE) != 0; }   // as it was when the tick began
-  if (!TRACE && !STAGED && !((busy & 7u) != 0 || pre.any != 0 || p.reap_now != 0 || timers_due)) { mind = min(mind, sleeping); if (due && (busy & 8u)) SFS_PROBE(20); return false; }
+  if (!TRACE && !STAGED && !(busy_business<PASS>(busy) != 0 || pre.any != 0 || p.reap_now != 0 || timers_due)) { mind = min(mind, sleeping); if (due && (busy & 8u)) SFS_PROBE(20); return false; }
   if (PASS && !due) cr = carry_of(p, vl);
   if (STAGED && !TRACE && !((busy & 7u) || (mL | mJ | mM) || p.reap_now || timers_due)) { mind = min(mind, sleeping); return false; }
   // (the watcher mask — subjects this node can probe, it has them as neighbours — is re-read where a watcher needs it: a handful of nodes)
@@ -860,7 +867,10 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
     for (int w = 0; w < BLOCK / 32; ++w) s += red[threadIdx.x][w];
     if (s) {
       if (threadIdx.x < 5) atomicAdd((unsigned long long*)(p.row + threadIdx.x), (unsigned long long)s);
-      else atomicAdd(p.kinds_cur + (threadIdx.x - 5), (u32)min(s, (u64)0xffffffffu));
+      else {
+        atomicAdd(p.kinds_cur + (threadIdx.x - 5), (u32)min(s, (u64)0xffffffffu));
+        if (PASS) atomicAdd(p.view_kinds_cur + (threadIdx.x - 5), (u32)min(s, (u64)0xffffffffu));   // a pass counts its own view only
+      }
     }
   }
   if (TRACE && lane == 0 && hs) atomicAdd((unsigned long long*)(p.row + 7), (unsigned long long)hs);
@@ -960,7 +970,10 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   }
   if (threadIdx.x == 0) dsusp_s = 0;                       // ordered before its first use by the barrier after the tile scan
   Counters c = {};
-  const bool kL = p.kinds_prev[KIND_LEAVE] != 0, kJ = p.kinds_prev[KIND_JOIN] != 0, kM = p.kinds_prev[KIND_ML] != 0;
+  // What this launch loads: the inbox planes of the kinds in flight, and (below) whether every node is requested up front.  A pass decides
+  // from its own view's traffic (view_kinds_prev, tick_kernel.cuh): a plane no sender of its view wrote is zero and stays unread.
+  const u32* const kv = PASS ? p.view_kinds_prev : p.kinds_prev;
+  const bool kL = kv[KIND_LEAVE] != 0, kJ = kv[KIND_JOIN] != 0, kM = kv[KIND_ML] != 0;
   const u64 pol_first = policy_evict_first(), pol_last = policy_evict_last();
   const int lane = threadIdx.x & 31;
   if (SHARDED && threadIdx.x < (BLOCK / 32) * MAX_WORLD) xs->cnt[threadIdx.x / MAX_WORLD][threadIdx.x % MAX_WORLD] = 0;
@@ -975,8 +988,14 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   const bool dense_now = prev_msgs >= (p.n_tiles >> 1) + 1;      // what this tick's sends will look like
   const bool all_hot = p.force_all || p.kinds_prev[3] != 0;      // the previous tick was dense (or skipping is off)
   const bool mark = !dense_now;
-  const bool saturated = prev_msgs >= (p.n_local >> 1);          // most nodes have mail: request record + node word up front
+  const u32 own_msgs = PASS ? kv[KIND_LEAVE] + kv[KIND_JOIN] + kv[KIND_ML] : prev_msgs;
+  const bool saturated = own_msgs >= (p.n_local >> 1);           // most nodes have mail: request record + node word up front
   if (dense_now && blockIdx.x == 0 && threadIdx.x == 0) p.kinds_cur[3] = 1;
+  if (PASS && work && threadIdx.x == 0) {                        // coverage of the host build: decisions the whole-tick counters would have taken otherwise
+    if (kv == p.kinds_prev) SFS_PROBE(23);                       // whole-tick fallback (an earlier writer of the inbox was not a pass)
+    if (!saturated && prev_msgs >= (p.n_local >> 1) && p.compact) SFS_PROBE(24);   // compacted walk in a tick another view saturates
+    if ((!kL && p.kinds_prev[KIND_LEAVE]) || (!kJ && p.kinds_prev[KIND_JOIN]) || (!kM && p.kinds_prev[KIND_ML])) SFS_PROBE(25);   // a plane of a kind in flight elsewhere, not read
+  }
 
   const u32 tile0 = blockIdx.x * p.tiles_per_cta;
   const u32 ntile = tile0 < p.n_tiles ? min(p.tiles_per_cta, p.n_tiles - tile0) : 0;
@@ -1019,7 +1038,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
         const bool due_g = g < ng && (hot_s[gt_s[g]] & 2u) != 0;
         Pre prg = pr[g];
         if (due_g && (prg.busy & 8u)) prg.nd = p.node_due[((tile0 + gt_s[g]) << TILE_SHIFT) + threadIdx.x];
-        const bool act = g < ng && node_active(p, prg, due_g);   // lanes past n_local hold an empty Pre
+        const bool act = g < ng && node_active<PASS>(p, prg, due_g);   // lanes past n_local hold an empty Pre
         if (due_g) {                                         // (warp-uniform) nodes whose own timers run later hand their deadline back to the wheel
           const u32 wm = warp_min(act ? NO_DEADLINE : sleeping_deadline(prg, true));
           if (lane == 0 && wm != NO_DEADLINE) atomicMin(p.tile_due + tile0 + gt_s[g], wm);

@@ -129,6 +129,10 @@ struct TickParams {
   u32 ahead;                  // multi-slot runs: 1 = saturated ticks request node word, peers and the probable first view's record one tile ahead; 2 = every tick (tests); 0 = off (SERFSIM_AHEAD)
   u32* host_idle_until;       // SCHED_IDLE_UNTIL mirrored into mapped pinned host memory: serfsim_run_until_converged does not even launch the ticks the cluster sleeps through
   u32* carry;                 // [stride] per-view passes (SV_PASS): what the earlier passes of the tick did at the node (CARRY_*)
+  // Per-view passes: the kind counters a pass chooses its loads from (which inbox planes it streams, whether it requests every node up
+  // front) — its own view's messages of the previous tick when every inbox write of that tick came from passes, the whole tick's
+  // (kinds_prev) otherwise; and its view's entry of this tick, which it adds its sends to.  Tile decisions stay whole-tick.
+  const u32* view_kinds_prev; u32* view_kinds_cur;
 };
 constexpr u32 SCHED_TICKET = 0, SCHED_IDLE_UNTIL = 1, SCHED_UE_ACTIVITY = 2, SCHED_AWAKE = 3, SCHED_SUSPECTS = 4 /* u64 */,
               SCHED_LOCAL_QUIET = 6, SCHED_LOCAL_UNTIL = 7 /* sharded runs: this rank's verdict; the drain kernel combines the ranks' */,

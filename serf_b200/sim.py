@@ -143,6 +143,7 @@ PRODUCT_ONLY = {
     "serfsim_last_step_device_ms": (C.c_int, [_vp, C.POINTER(C.c_double), C.POINTER(_u64)]),
     "serfsim_set_tick_timing": (C.c_int, [_vp, C.c_int]),
     "serfsim_tick_times": (C.c_int, [_vp, _u32, _u32, _vp]),
+    "serfsim_tick_view_kinds": (C.c_int, [_vp, _u32, _u32, _vp]),
     "serfsim_comm_blob_size": (C.c_size_t, []),
     "serfsim_comm_export": (C.c_int, [_vp, _vp]),
     "serfsim_comm_connect": (C.c_int, [_vp, _vp]),
@@ -417,6 +418,15 @@ class GossipSim:
         out = np.zeros(n, dtype=np.float32)
         if n:
             self._check(self._lib.serfsim_tick_times(self._h, int(first), int(n), out.ctypes.data))
+        return out
+
+    def tick_view_kinds(self, first=0, n=None):
+        """[n, slots, 3] messages (leave, join, memberlist) each view sent per tick, counted by the per-view passes (zero in ticks without)."""
+        if n is None:
+            n = self.stats()["tick"] - first
+        out = np.zeros((n, self.slots, 3), dtype=np.uint32)
+        if n:
+            self._check(self._lib.serfsim_tick_view_kinds(self._h, int(first), int(n), out.ctypes.data))
         return out
 
     def set_event_callback(self, fn):
