@@ -319,7 +319,10 @@ int serfsim_wire_decode_push_pull(const uint8_t* buf, size_t len, serfsim_wire_p
  * fails after setting *total.  A virtual node's member table holds the tracked subjects it knows. */
 int serfsim_wire_local_state_batch(serfsim_t* h, uint8_t* out, size_t cap, uint64_t* offsets, size_t* total);
 /* The inverse batch on the device: n concatenated push-pull messages → per message the Lamport clock and up to `cap`
- * (id, status_time) entries (arrays [n][cap]) with their count. */
+ * (id, status_time) entries (arrays [n][cap]) with their count.  Offsets: offsets has n + 1 entries; message i is
+ * buf[offsets[i] .. offsets[i + 1]); buf holds at least offsets[n] bytes (they are copied to the device).  Offsets that
+ * decrease fail the call with SERFSIM_E_INVAL before anything runs, naming the first bad index.  A malformed message fails
+ * the call, naming the lowest such index; a message with more than 16 (MAX_SLOTS) left_members entries counts as one. */
 int serfsim_wire_decode_batch(serfsim_t* h, const uint8_t* buf, const uint64_t* offsets, uint32_t n, uint32_t cap,
                               uint64_t* ltime, uint64_t* ids, uint64_t* status_ltimes, uint32_t* n_status);
 
@@ -361,7 +364,9 @@ int serfsim_wire_local_state_range(serfsim_t* h, uint32_t first, uint32_t count,
 /* The rings of n concatenated push-pull messages back to the simulator's form, on the device: per message its event clock
  * (event_ltime), the mask of tracked events its ring holds (bit e: a UserEvent with e's name and payload in an entry whose
  * ltime is e's Lamport time; tracked events with equal content and ltime resolve to the lowest index) and the number of
- * events that match no tracked event.  Needs a content table.  A malformed message fails the call (index in the error text). */
+ * events that match no tracked event.  Needs a content table.  Offsets as for serfsim_wire_decode_batch: n + 1 non-decreasing
+ * entries, buf holding at least offsets[n] bytes; decreasing offsets fail the call with SERFSIM_E_INVAL before anything
+ * runs.  A malformed message fails the call, naming the lowest such index. */
 int serfsim_wire_decode_events_batch(serfsim_t* h, const uint8_t* buf, const uint64_t* offsets, uint32_t n,
                                      uint64_t* event_ltime, uint32_t* seen, uint32_t* n_unmatched);
 

@@ -352,6 +352,16 @@ int encode_pp(const serfsim_wire_push_pull_t* m, const serfsim_wire_user_events_
   return o == need ? 0 : serfsim_fail(SERFSIM_E_INVAL, "wire: internal length mismatch");
 }
 
+// The batch decoders copy offsets[n] bytes of `buf` to the device and give message i the slice [offsets[i], offsets[i + 1]):
+// non-decreasing offsets keep every slice inside those bytes.  Checked before anything is allocated or launched.
+int check_batch_offsets(const uint64_t* offsets, u32 n) {
+  for (u32 i = 0; i < n; ++i)
+    if (offsets[i] > offsets[i + 1])
+      return serfsim_fail(SERFSIM_E_INVAL, (std::string("wire: offsets[") + std::to_string(i) + "] > offsets[" + std::to_string(i + 1) + "]: message " +
+                                            std::to_string(i) + " would end before it starts").c_str());
+  return 0;
+}
+
 }  // namespace
 
 #pragma GCC visibility push(default)
@@ -457,6 +467,8 @@ int serfsim_wire_decode_batch(serfsim_t* h, const uint8_t* buf, const uint64_t* 
   WireView v{};
   int rc = serfsim_wire_view(h, &v);
   if (rc) return rc;
+  if ((rc = check_batch_offsets(offsets, n))) return rc;
+  if (!n) return 0;                                          // nothing to decode
   const size_t total = (size_t)offsets[n];
   u8* d_buf = nullptr; u64 *d_off = nullptr, *d_lt = nullptr, *d_ids = nullptr, *d_sts = nullptr; u32 *d_ns = nullptr, *d_err = nullptr;
   auto cleanup = [&]() { cudaFree(d_buf); cudaFree(d_off); cudaFree(d_lt); cudaFree(d_ids); cudaFree(d_sts); cudaFree(d_ns); cudaFree(d_err); };
@@ -550,6 +562,8 @@ int serfsim_wire_decode_events_batch(serfsim_t* h, const uint8_t* buf, const uin
   int rc = serfsim_wire_view(h, &v);
   if (rc) return rc;
   if (!v.ue.n) return serfsim_fail(SERFSIM_E_INVAL, "wire: no user-event content table (serfsim_set_user_event_content)");
+  if ((rc = check_batch_offsets(offsets, n))) return rc;
+  if (!n) return 0;                                          // nothing to decode
   const size_t total = (size_t)offsets[n];
   u8* d_buf = nullptr; u64 *d_off = nullptr, *d_ev = nullptr; u32 *d_seen = nullptr, *d_um = nullptr, *d_err = nullptr;
   auto cleanup = [&]() { cudaFree(d_buf); cudaFree(d_off); cudaFree(d_ev); cudaFree(d_seen); cudaFree(d_um); cudaFree(d_err); };

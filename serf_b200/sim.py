@@ -374,6 +374,10 @@ class GossipSim:
         seen uint32[n] — bit e: tracked event e is in the ring —, unmatched uint32[n] — events matching no tracked event)."""
         buf = np.ascontiguousarray(buf, dtype=np.uint8)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        if offsets.ndim != 1 or offsets.size == 0 or offsets.size > 2**32:
+            raise ValueError("offsets must be a 1-D array of n + 1 entries, 0 <= n < 2**32")
+        if int(offsets[-1]) > buf.size:
+            raise ValueError(f"offsets[-1] = {int(offsets[-1])} is past the end of the {buf.size}-byte buffer")
         n = offsets.size - 1
         ev, seen, um = np.zeros(n, np.uint64), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
         self._check(self._lib.serfsim_wire_decode_events_batch(self._h, buf.ctypes.data, offsets.ctypes.data, n, ev.ctypes.data,

@@ -1,5 +1,6 @@
 """An independent restatement, in Python, of user events on serf's wire — test infrastructure, the checker of the user-event
-half of serf_b200/csrc/wire.cuh / wire_codec.cu.
+half of serf_b200/csrc/wire.cuh / wire_codec.cu, and the third decoder (beside the product and oracle/wire_oracle.cpp) of
+Join / Leave / PushPull that tests/test_wire_malformed.py compares on malformed bytes.
 
 Follows serf-core/src/types: user_event.rs (UserEvent: name = 1, payload = 2, LengthDelimited, each written only when
 non-empty, both default to empty, a second one is a duplicate), user_event/user_events.rs (UserEvents: ltime = 1 Varint
@@ -51,12 +52,18 @@ def get_varint(b, o):
     raise WireError("varint")
 
 
-def fields(b):
-    """(tag byte, value) for every field of a TLV stream: int for Varint / Byte, bytes for LengthDelimited."""
-    o = 0
+def fields(b, once=None):
+    """(tag byte, value) for every field of a TLV stream: int for Varint / Byte, bytes for LengthDelimited.  once: tag byte →
+    group of the fields that may appear once; a second field of a group is a duplicate, reported before its value is read
+    (the `if x.is_some() { return Err(duplicate_field) }` that opens every singular arm, e.g. join.rs:68-75, message.rs:520-527)."""
+    o, seen = 0, set()
     while o < len(b):
         t = b[o]
         w = t & 7
+        if once and t in once:
+            if once[t] in seen:
+                raise WireError("duplicate")
+            seen.add(once[t])
         o += 1
         if w == BYTE:
             if o >= len(b):
@@ -120,38 +127,54 @@ def push_pull(ltime, status, left, event_ltime, ring, query_ltime):
 
 
 # ---- decoders (raise WireError) ----
+def _once(*tags):
+    return {t: t for t in tags}
+
+
 def open_envelope(b):
     found = None
-    for t, v in fields(b):
+    for t, v in fields(b, once={t: "message" for t in MSG_BYTES}):          # one message per buffer (message.rs:520-527)
         if t in MSG_BYTES:
-            if found is not None:
-                raise WireError("duplicate")
             found = (t >> 3, v)
     if found is None:
         raise WireError("missing")
     return found
 
 
+def d_intent(b):
+    """JoinMessage::decode (join.rs:54-105) / LeaveMessage::decode (leave.rs:56-119) with the envelope: (kind, ltime, id,
+    prune), kind 1 = leave, 2 = join.  A second Join id is a duplicate; a second Leave id replaces the first."""
+    kind, body = open_envelope(b)
+    if kind not in (1, 2):
+        raise WireError("type")
+    leave = kind == 1
+    if leave:                                                  # leave.rs:8-13: ltime = 1, prune = 2 (Byte), id = 3
+        keys, once = {tag(VARINT, 1): "ltime", tag(BYTE, 2): "prune", tag(VARINT, 3): "id"}, _once(tag(VARINT, 1), tag(BYTE, 2))
+    else:                                                      # join.rs:8-10: ltime = 1, id = 2
+        keys, once = {tag(VARINT, 1): "ltime", tag(VARINT, 2): "id"}, _once(tag(VARINT, 1), tag(VARINT, 2))
+    got = {}
+    for t, v in fields(body, once=once):
+        if t in keys:
+            got[keys[t]] = v
+    if "ltime" not in got or "id" not in got:
+        raise WireError("missing")
+    return kind, got["ltime"], got["id"], bool(got.get("prune", 0))
+
+
 def d_user_event(b):
     name = payload = None
-    for t, v in fields(b):
+    for t, v in fields(b, once=_once(tag(LEN, 1), tag(LEN, 2))):
         if t == tag(LEN, 1):
-            if name is not None:
-                raise WireError("duplicate")
             name = v
         elif t == tag(LEN, 2):
-            if payload is not None:
-                raise WireError("duplicate")
             payload = v
     return name or b"", payload or b""
 
 
 def d_user_events(b):
     lt, evs = None, []
-    for t, v in fields(b):
+    for t, v in fields(b, once=_once(tag(VARINT, 1))):
         if t == tag(VARINT, 1):
-            if lt is not None:
-                raise WireError("duplicate")
             lt = v
         elif t == tag(LEN, 2):
             evs.append(d_user_event(v))
@@ -164,14 +187,11 @@ def d_user_event_message(b):
     kind, body = open_envelope(b)
     if kind != 4:
         raise WireError("type")
+    keys = {tag(VARINT, 1): "ltime", tag(BYTE, 2): "cc", tag(LEN, 3): "name", tag(LEN, 4): "payload"}
     got = {}
-    for t, v in fields(body):
-        key = {tag(VARINT, 1): "ltime", tag(BYTE, 2): "cc", tag(LEN, 3): "name", tag(LEN, 4): "payload"}.get(t)
-        if key is None:
-            continue
-        if key in got:
-            raise WireError("duplicate")
-        got[key] = v
+    for t, v in fields(body, once=_once(*keys)):
+        if t in keys:
+            got[keys[t]] = v
     if "ltime" not in got:
         raise WireError("missing")
     return got["ltime"], got.get("name", b""), got.get("payload", b""), bool(got.get("cc", 0))
@@ -182,10 +202,8 @@ def d_push_pull(b):
     if kind != 3:
         raise WireError("type")
     one, status, left, ring = {}, [], [], []
-    for t, v in fields(body):
+    for t, v in fields(body, once=_once(tag(VARINT, 1), tag(VARINT, 4), tag(VARINT, 6))):
         if t in (tag(VARINT, 1), tag(VARINT, 4), tag(VARINT, 6)):
-            if t in one:
-                raise WireError("duplicate")
             one[t] = v
         elif t == tag(LEN, 2):
             kv = dict((tt, vv) for tt, vv in fields(v) if tt in (tag(VARINT, 1), tag(VARINT, 2)))

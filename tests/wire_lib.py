@@ -134,10 +134,20 @@ def local_state_batch(L, sim):
     return out[:tot.value], off
 
 
-def decode_batch(L, sim, buf, off, cap):
-    n = len(off) - 1
+def decode_batch(L, sim, buf, off, cap, check=True):
+    """serfsim_wire_decode_batch over message i = buf[off[i]:off[i + 1]].  check=False returns (rc, outputs) instead of
+    asserting success."""
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    if off.ndim != 1 or off.size == 0:
+        raise ValueError("offsets must be a 1-D array of n + 1 entries")
+    if int(off[-1]) > buf.size:
+        raise ValueError(f"offsets[-1] = {int(off[-1])} is past the end of the {buf.size}-byte buffer")
+    n = off.size - 1
     lt, ids, sts, ns = np.zeros(n, np.uint64), np.zeros((n, cap), np.uint64), np.zeros((n, cap), np.uint64), np.zeros(n, np.uint32)
-    rc = L.serfsim_wire_decode_batch(sim._h, np.ascontiguousarray(buf).ctypes.data, off.ctypes.data, n, cap, lt.ctypes.data, ids.ctypes.data, sts.ctypes.data, ns.ctypes.data)
+    rc = L.serfsim_wire_decode_batch(sim._h, buf.ctypes.data, off.ctypes.data, n, cap, lt.ctypes.data, ids.ctypes.data, sts.ctypes.data, ns.ctypes.data)
+    if not check:
+        return rc, (lt, ids, sts, ns)
     assert rc == 0, rc
     return lt, ids, sts, ns
 

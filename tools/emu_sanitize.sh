@@ -18,5 +18,5 @@ cd "$ROOT"
   LD_PRELOAD="$(g++ -print-file-name=libasan.so) $(g++ -print-file-name=libubsan.so)" \
   ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
   SERFSIM_EMU_LIB=$W/libserfsim_emu_asan.so python -m pytest tests/test_emu_parity.py tests/test_emu_multi.py tests/test_emu_uevent.py \
-      tests/test_emu_byzantine.py tests/test_emu_host.py tests/test_golden_features.py -q -s 2>&1 | grep -v "^\.*$" | tail -20
+      tests/test_emu_byzantine.py tests/test_emu_host.py tests/test_golden_features.py tests/test_wire_malformed.py -q -s 2>&1 | grep -v "^\.*$" | tail -20
 } > "$OUT"
