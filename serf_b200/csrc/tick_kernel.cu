@@ -198,7 +198,7 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
   if (!SHARDED || dl < p.n_local) {
     if (val1 > held) red_max_resident(plane + dl, val1, pol_last);
     else SFS_PROBE(22);
-    if (mark) p.hot_wr[dl >> TILE_SHIFT] = 1;  // sparse ticks only: tell the next tick which tiles received something
+    if (mark) { p.hot_wr[dl >> TILE_SHIFT] = 1; SFS_PROBE(26); }   // sparse ticks only: tell the next tick which tiles received something
   } else {
     u32 dloc;
     const u32 shard = shard_of(p, dst, dloc);
@@ -480,6 +480,7 @@ __device__ SFS_COLD void cold_reap(Rec& r, u32 t, u32 tombstone, u32 reconnect, 
   const u32 age = r.leave_tick ? (t + 1 - r.leave_tick) : 0;
   if ((r.flags & 1) && r.leave_tick && ((r.status == ST_LEFT && age > tombstone) || (r.status == ST_FAILED && age > reconnect))) {
     r.flags &= ~1u; r.status = TY_NONE; r.st = 0; r.leave_tick = 0;           // erase_node! :499-519
+    SFS_PROBE(27);
   } else if (!(r.flags & 1) && r.status != TY_NONE && r.leave_tick && age > intent) {
     r.status = TY_NONE; r.st = 0; r.leave_tick = 0;                           // reap_intents :1817-1822
   }
@@ -1325,7 +1326,7 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
         p.rec[2 * iv] = a1; p.rec[2 * iv + 1] = bs;
         if (q1 != q0) p.qword[iv] = q1;
       }
-      if ((a1.y ^ a0.y) | (a1.z ^ a0.z) | (a1.w ^ a0.w) | (b1.x ^ b0.x) | (b1.y ^ b0.y) | (b1.z ^ b0.z) | (b1.w ^ b0.w)) d_changed++;   // status_time creep is not a change
+      if ((a1.y ^ a0.y) | (a1.z ^ a0.z) | (a1.w ^ a0.w) | (b1.x ^ b0.x) | (b1.y ^ b0.y) | (b1.z ^ b0.z) | (b1.w ^ b0.w)) { d_changed++; SFS_PROBE(28); }   // status_time creep is not a change
       if (TRACE && ch) d_hash += rec_hash((u64)s * p.n_global + v, a1, b1) - rec_hash((u64)s * p.n_global + v, a0, b0);
       const bool watching = p.probe_every && ((p.down_mask >> s) & 1) && !self && ((wmask >> s) & 1);
       const bool now = (r.txl | r.txj | r.txm) || r.mlstate == ML_SUSPECT || (watching && r.mlstate == ML_ALIVE);

@@ -9,7 +9,8 @@ test infrastructure only.
   graphs.
 - kernel_lines: the kernel and grid the library prints for each topology under SERFSIM_VERBOSE.
 - run_isolated: runs of the product library in a fresh process.  SERFSIM_GRIDMUL, SERFSIM_MINB and SERFSIM_TMA_SYNC are read
-  once per process (the first launch fixes them), so a variant selected by them only runs in a process of its own.
+  once per process (the first launch fixes them), so a variant selected by them only runs in a process of its own.  Its outputs
+  include the user-event and injector outputs (feature_outputs) and the per-view kind counters.
 """
 import os
 import pickle
@@ -195,6 +196,18 @@ def _outputs(sim, slots):
     return out
 
 
+def feature_outputs(sim, sc):
+    """The user-event and injector outputs of a run of `sc` (empty when the scenario has neither)."""
+    out = {}
+    if sc.user_events is not None:
+        out.update(ue_records=sim.user_event_records(), ue_stats=sim.user_event_stats(), ue_event_time=sim.event_time(),
+                   ue_ltime=[sim.user_event_ltime(e) for e in range(len(sc.user_events))],
+                   ue_seen=[sim.user_event_seen(e) for e in range(len(sc.user_events))])
+    if sc.byzantine is not None:
+        out.update(byz_stats=sim.byzantine_stats(), anomaly=sim.anomaly_flags())
+    return out
+
+
 def _child(job_path, out_path):
     from serf_b200 import GossipSim, sim as _sim
     if ON_EMU:
@@ -216,7 +229,7 @@ def _child(job_path, out_path):
         g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), trace=trace, **job.get("cfg", {}))
         r = g.run_until_converged(sc.max_ticks)
         out = _outputs(g, sc.slots)
-        out["run"] = r
+        out.update(feature_outputs(g, sc), run=r, view_kinds=g.tick_view_kinds())
         g.close()
         res.append(out)
     with open(out_path, "wb") as f:
