@@ -8,9 +8,9 @@ test infrastructure only.
 - envelope_fuzz: scenarios.fuzz over the whole fan-out (1–8) and slot (1–16) range, on regular, small-world or irregular
   graphs.
 - kernel_lines: the kernel and grid the library prints for each topology under SERFSIM_VERBOSE.
-- run_isolated: runs of the product library in a fresh process.  SERFSIM_GRIDMUL, SERFSIM_MINB and SERFSIM_TMA_SYNC are read
-  once per process (the first launch fixes them), so a variant selected by them only runs in a process of its own.  Its outputs
-  include the user-event and injector outputs (feature_outputs) and the per-view kind counters.
+- product_run: a run's parity outputs (parity_lib.outputs) with the product-only getters beside them.
+- run_isolated: product_run in a fresh process.  SERFSIM_GRIDMUL, SERFSIM_MINB and SERFSIM_TMA_SYNC are read once per process (the
+  first launch fixes them), so a variant selected by them only runs in a process of its own.
 """
 import os
 import pickle
@@ -25,6 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+import parity_lib as P                                                       # noqa: E402
 from serf_b200 import scenarios                                              # noqa: E402
 from serf_b200.scenarios import Scenario                                     # noqa: E402
 from serf_b200.sim import Op, random_regular_graph, small_world_graph         # noqa: E402
@@ -182,30 +183,12 @@ def busy_ctas(n, grid):
     return (tiles + per - 1) // per
 
 
-# ---- runs in a fresh process --------------------------------------------------------------------------------
-def _outputs(sim, slots):
-    out = dict(stats=sim.stats(), trace=sim.tick_trace(), hash=sim.state_hash(), clock=sim.lamport_time(),
-               clock32=sim.lamport_time_u32(), launches=sim.last_step_device_ms()[1])
-    for s in range(slots):
-        out[f"rec{s}"] = sim.records(s)
-        out[f"status{s}"] = sim.member_status(s)
-        out[f"sltime{s}"] = sim.status_ltime(s)
-        out[f"sltime32_{s}"] = sim.status_ltime_u32(s)
-        out[f"inc{s}"] = sim.incarnation(s)
-        out[f"ml{s}"] = sim.ml_state(s)
-    return out
-
-
-def feature_outputs(sim, sc):
-    """The user-event and injector outputs of a run of `sc` (empty when the scenario has neither)."""
-    out = {}
-    if sc.user_events is not None:
-        out.update(ue_records=sim.user_event_records(), ue_stats=sim.user_event_stats(), ue_event_time=sim.event_time(),
-                   ue_ltime=[sim.user_event_ltime(e) for e in range(len(sc.user_events))],
-                   ue_seen=[sim.user_event_seen(e) for e in range(len(sc.user_events))])
-    if sc.byzantine is not None:
-        out.update(byz_stats=sim.byzantine_stats(), anomaly=sim.anomaly_flags())
-    return out
+# ---- runs of the product -------------------------------------------------------------------------------------
+def product_run(sim, sc):
+    """Runs sim (built from sc) to convergence: {"out": its parity outputs, "view_kinds": the per-view kind counters, "launches":
+    the kernel launches of the last step call}."""
+    out = P.outputs(sim, sc, sim.run_until_converged(sc.max_ticks))
+    return dict(out=out, view_kinds=sim.tick_view_kinds(), launches=sim.last_step_device_ms()[1])
 
 
 def _child(job_path, out_path):
@@ -226,12 +209,9 @@ def _child(job_path, out_path):
             res.append(None)
             continue
         sc, trace = job["sc"], job["trace"]
-        g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), trace=trace, **job.get("cfg", {}))
-        r = g.run_until_converged(sc.max_ticks)
-        out = _outputs(g, sc.slots)
-        out.update(feature_outputs(g, sc), run=r, view_kinds=g.tick_view_kinds())
+        g = sc.build(GossipSim, trace=trace, **job.get("cfg", {}))
+        res.append(product_run(g, sc))
         g.close()
-        res.append(out)
     with open(out_path, "wb") as f:
         pickle.dump(res, f)
 
@@ -239,7 +219,7 @@ def _child(job_path, out_path):
 def run_isolated(jobs, env=None, timeout=1200):
     """Run jobs — dict(sc=Scenario, trace=0/1, cfg={...}) or dict(probe=n) — through the product library (the host build under
     SERFSIM_GPU_TESTS_ON_EMU=1) in a new Python process with `env` added to this one's and SERFSIM_VERBOSE=1.
-    Returns one dict of outputs per job; its "kernel" is (kernel name, grid) of the job's topology (kernel_lines)."""
+    Returns one product_run dict per job, with "kernel": (kernel name, grid) of the job's topology (kernel_lines)."""
     e = dict(os.environ)
     e.update(env or {})
     e["SERFSIM_VERBOSE"] = "1"
@@ -261,33 +241,6 @@ def run_isolated(jobs, env=None, timeout=1200):
 def grid_for(n, env=None):
     """(kernel name, grid) the library picks for an n-node single-slot handle under `env`."""
     return run_isolated([dict(probe=n)], env)[0]["kernel"]
-
-
-def assert_matches(got, o, slots, with_hash, what=""):
-    """got: outputs of a run (run_isolated); o: the oracle after the same run with trace = 1.  Everything the parity tests
-    compare: stats, every trace row (the hash only when the run had trace = 1), clocks, every slot's records and getters, state hash."""
-    so = o.stats()
-    assert got["stats"] == so, (what, got["stats"], so)
-    n = so["tick"]
-    tg, to = got["trace"][:n], o.tick_trace(0, n)
-    assert got["trace"].size == n
-    for f in to.dtype.names:
-        if f == "hash" and not with_hash:
-            continue
-        bad = np.nonzero(tg[f] != to[f])[0]
-        assert bad.size == 0, f"{what}: trace field {f} first differs at tick {bad[0]}: device {tg[f][bad[0]]} oracle {to[f][bad[0]]}"
-    oc = o.lamport_time()
-    assert (got["clock"] == oc).all() and (got["clock32"] == oc).all(), what
-    for s in range(slots):
-        ro = o.records(s)
-        bad = np.nonzero(got[f"rec{s}"] != ro)[0]
-        assert bad.size == 0, f"{what}: slot {s}: record of node {bad[0]} differs: device {got[f'rec{s}'][bad[0]]} oracle {ro[bad[0]]}"
-        assert (got[f"status{s}"] == o.member_status(s)).all(), what
-        lt = o.status_ltime(s)
-        assert (got[f"sltime{s}"] == lt).all() and (got[f"sltime32_{s}"] == lt).all(), what
-        assert (got[f"inc{s}"] == o.incarnation(s)).all(), what
-        assert (got[f"ml{s}"] == o.ml_state(s)).all(), what
-    assert got["hash"] == o.state_hash(), what
 
 
 if __name__ == "__main__":

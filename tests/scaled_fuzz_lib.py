@@ -9,8 +9,6 @@ saturates and another does not, sleeping stretches the scheduler skips or jumps 
 
 - scaled_fuzz(seed, n=None): the scenario.  Every draw comes from Philox streams of the seed, so a seed gives the same scenario on every
   machine; `n` replaces the drawn node count (the ragged last tile is still drawn, so n is rounded to a multiple of 256 plus 1 – 255).
-- outputs / oracle_outputs / assert_same_outputs: everything a run computes — stats, trace rows, clocks, every slot's records and
-  getters, the state hash, user-event records / stats / clocks / seen vectors, injector stats and anomaly flags — and the comparison.
 - reach: which production paths a trace = 0 run of the product took, derived from its getters alone (no probes on the device).
 """
 import math
@@ -161,67 +159,15 @@ def scaled_fuzz(seed, n=None):
     return sc
 
 
-# ---- what a run computed, and the comparison ------------------------------------------------------------------------
-def oracle_outputs(o, sc, run):
-    """The oracle's outputs (its run had trace = 1), in the keys of outputs()."""
-    out = dict(run=run, stats=o.stats(), trace=o.tick_trace(), hash=o.state_hash(), clock=o.lamport_time())
-    out["clock32"] = out["clock"]
-    for s in range(sc.slots):
-        out[f"rec{s}"] = o.records(s)
-        out[f"status{s}"] = o.member_status(s)
-        out[f"sltime{s}"] = out[f"sltime32_{s}"] = o.status_ltime(s)
-        out[f"inc{s}"] = o.incarnation(s)
-        out[f"ml{s}"] = o.ml_state(s)
-    out.update(E.feature_outputs(o, sc))
-    return out
-
-
-def outputs(sim, sc, run):
-    """The product's (or the host build's) outputs after a run; `view_kinds` and `launches` are product-only getters."""
-    out = E._outputs(sim, sc.slots)
-    out.update(E.feature_outputs(sim, sc), run=run, view_kinds=sim.tick_view_kinds())
-    return out
-
-
-def assert_same_outputs(got, ref, sc, with_hash, what=""):
-    assert got["run"] == ref["run"], (what, got["run"], ref["run"])
-    assert got["stats"] == ref["stats"], (what, got["stats"], ref["stats"])
-    n = ref["stats"]["tick"]
-    tg, to = got["trace"][:n], ref["trace"][:n]
-    assert got["trace"].size == n, what
-    for f in to.dtype.names:
-        if f == "hash" and not with_hash:
-            continue
-        bad = np.nonzero(tg[f] != to[f])[0]
-        assert bad.size == 0, f"{what}: trace field {f} first differs at tick {bad[0]}: got {tg[f][bad[0]]} oracle {to[f][bad[0]]}"
-    assert (got["clock"] == ref["clock"]).all() and (got["clock32"] == ref["clock"]).all(), what
-    for s in range(sc.slots):
-        bad = np.nonzero(got[f"rec{s}"] != ref[f"rec{s}"])[0]
-        assert bad.size == 0, f"{what}: slot {s}: record of node {bad[0]} differs: got {got[f'rec{s}'][bad[0]]} oracle {ref[f'rec{s}'][bad[0]]}"
-        for k in ("status", "sltime", "sltime32_", "inc", "ml"):
-            assert (got[f"{k}{s}"] == ref[f"{k}{s}"]).all(), (what, k, s)
-    assert got["hash"] == ref["hash"], what
-    for k in ("ue_records", "ue_event_time", "anomaly"):
-        if k in ref:
-            bad = np.nonzero(got[k] != ref[k])[0]
-            assert bad.size == 0, f"{what}: {k} of node {bad[0]} differs: got {got[k][bad[0]]} oracle {ref[k][bad[0]]}"
-    for k in ("ue_stats", "ue_ltime", "byz_stats"):
-        if k in ref:
-            assert got[k] == ref[k], (what, k, got[k], ref[k])
-    if "ue_seen" in ref:
-        for e, seen in enumerate(ref["ue_seen"]):
-            assert (got["ue_seen"][e] == seen).all(), (what, "user_event_seen", e)
-
-
 # ---- which production paths a trace = 0 run took, from the product's getters ----------------------------------------
 def reach(got, sc):
-    """Counts of the ticks of a trace = 0 run that exercised each path, from the trace rows and the per-view kind counters.
+    """got: an envelope_lib.product_run of sc.  Counts of the ticks of a trace = 0 run that exercised each path, from the trace rows and the per-view kind counters.
     pass_ticks: ticks that ran as per-view passes.  compacted_under_other: pass ticks after a pass tick in which the whole tick sent
     at least n / 2 messages but some view fewer (that view's pass takes the compacted walk).  unread_plane: pass ticks after a pass
     tick in which a kind was in flight in one view and absent in another.  sparse / dense: ticks below / at or above tiles / 2 messages."""
     n = sc.n
     tiles = (n + TILE - 1) // TILE
-    msgs = got["trace"]["messages"].astype(np.int64)
+    msgs = got["out"]["trace"]["messages"].astype(np.int64)
     vk = got["view_kinds"].astype(np.int64)
     ran = vk.reshape(len(vk), -1).sum(axis=1) > 0
     follow = ran[1:] & ran[:-1]                                    # tick t + 1 ran as passes on the counts of pass tick t

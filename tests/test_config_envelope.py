@@ -14,13 +14,12 @@ import numpy as np
 import pytest
 
 import config_lib as CL
+import parity_lib as P
 from emu_lib import emu_sim
 from oracle_lib import lib as olib, oracle_sim
 from serf_b200 import MlState, scenarios
 from serf_b200.scenarios import Op, Scenario
 from serf_b200.sim import SerfsimError, full_mesh_graph, random_regular_graph
-from test_emu_multi import ThreadComm, check as check_sharded
-from test_emu_parity import assert_same, run_both
 
 E_INVAL, E_OVERFLOW = -1, -5
 
@@ -137,7 +136,7 @@ def _parity_or_overflow(sc):
     o = sc.build(oracle_sim, trace=1)
     o.run_until_converged(sc.max_ticks)
     assert CL.max_ltime(o, sc.slots) < CL.LTIME_LIMIT, sc.name        # the draw keeps every run inside the device range
-    run_both(sc)
+    P.run_against_oracle(emu_sim, sc)
     return o
 
 
@@ -174,7 +173,7 @@ def test_config_fuzz_sharded_across_a_power_of_ten(seed, n):
     sc = CL.config_fuzz(seed, n=n)
     sc.max_ticks = 200
     assert CL.digits((n + 1) // 2) == CL.digits(n) - 1
-    check_sharded(sc, 2)
+    P.run_against_oracle(emu_sim, sc, world=2)
 
 
 # ---- validation ---------------------------------------------------------------------------------------------------
@@ -299,13 +298,10 @@ def assert_overflow_at(sc, trace, factory=emu_sim):
     assert k > 3, k                                            # the run starts inside the range and gets there by its own operations
     o = sc.build(oracle_sim, trace=1)
     g = sc.build(factory, trace=trace)
-    for _ in range(k - 1):
+    for i in range(k - 1):
         o.step(1)
         g.step(1)
-        assert (g.lamport_time() == o.lamport_time()).all()
-        for s in range(sc.slots):
-            assert (g.records(s) == o.records(s)).all()
-    assert_same(g, o, sc.slots, with_hash=bool(trace))
+        P.assert_same(P.outputs(g, sc, None), P.outputs(o, sc, None), with_hash=bool(trace), what=f"step {i + 1}")
     assert CL.max_ltime(g, sc.slots) < CL.LTIME_LIMIT
     with pytest.raises(SerfsimError) as ei:
         g.step(1)
@@ -349,7 +345,7 @@ def test_overflow_sharded_world_2():
     o = sc.build(oracle_sim, trace=1)
     o.step(k - 1)
     for trace in (1, 0):
-        comm, world = ThreadComm(2), 2
+        comm, world = P.ThreadComm(2), 2
         first_err, res, errs = [None, None], [None, None], []
 
         def worker(rank):
@@ -363,7 +359,7 @@ def test_overflow_sharded_world_2():
                         if first_err[rank] is None:
                             first_err[rank] = (i, e.code)
                     if i == k - 1:
-                        res[rank] = dict(clock=g.lamport_time(), rec=[g.records(s) for s in range(sc.slots)])
+                        res[rank] = P.outputs(g, sc, None)
                 comm.bar.wait()
             except BaseException as e:                    # noqa: BLE001 — surface it in the main thread
                 errs.append(e)
@@ -375,8 +371,6 @@ def test_overflow_sharded_world_2():
             t.join(600)
         if errs:
             raise errs[0]
-        assert (np.concatenate([r["clock"] for r in res]) == o.lamport_time()).all()
-        for s in range(sc.slots):
-            assert (np.concatenate([r["rec"][s] for r in res]) == o.records(s)).all()
+        P.assert_same(P.merge_ranks(res), P.outputs(o, sc, None), with_hash=bool(trace))
         got = [e for e in first_err if e is not None]
         assert got and all(e == (k, E_OVERFLOW) for e in got), (first_err, k)

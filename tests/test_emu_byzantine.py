@@ -1,52 +1,37 @@
 """Byzantine-injector kernel logic on the CPU: byz_kernel.cu (and the host code around it) compiled for the host by
 tests/emu, against the oracle's definition — the comparisons of tests/test_gpu_z_byzantine.py at small sizes."""
-import numpy as np
 import pytest
 
+import parity_lib as P
 from emu_lib import emu_sim
 from oracle_lib import oracle_sim
 from serf_b200 import scenarios
-from test_emu_parity import assert_same
-
-
-def run_both(sc, **cfg):
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    for trace in (1, 0):
-        g = sc.build(emu_sim, trace=trace, **cfg)
-        assert g.run_until_converged(sc.max_ticks) == to
-        assert_same(g, o, sc.slots, with_hash=bool(trace))
-        fg, fo = g.anomaly_flags(), o.anomaly_flags()
-        bad = np.nonzero(fg != fo)[0]
-        assert bad.size == 0, f"anomaly flag of node {bad[0]}: emu {fg[bad[0]]} oracle {fo[bad[0]]}"
-        assert g.byzantine_stats() == o.byzantine_stats()
-    return g, o
 
 
 @pytest.mark.parametrize("seed", [1, 2])
 def test_config4_shape_one_percent(seed):
     sc = scenarios.byzantine_injectors(5000, 16, 4, 0.01, seed=seed)
-    g, o = run_both(sc)
-    assert g.anomaly_flags()[sc.byzantine].mean() > 0.9
+    out = P.run_against_oracle(emu_sim, sc)
+    assert out["anomaly_flags"][sc.byzantine].mean() > 0.9
 
 
 def test_heavy_injection_changes_the_trace():
     sc = scenarios.byzantine_injectors(3000, 16, 4, 0.2, seed=3)
-    g, o = run_both(sc)
+    out = P.run_against_oracle(emu_sim, sc)
     honest = scenarios.byzantine_injectors(3000, 16, 4, 0.2, seed=3)
     honest.byzantine = None
     h = honest.build(oracle_sim, trace=1)
     h.run_until_converged(honest.max_ticks)
-    assert o.stats() != h.stats()                      # the stale copies did change the honest dynamics in this run
+    assert out["stats"] != h.stats()                      # the stale copies did change the honest dynamics in this run
 
 
 def test_single_slot_no_probing():
-    run_both(scenarios.byzantine_injectors(3000, 12, 3, 0.05, seed=2, churn=False, slots=1))
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(3000, 12, 3, 0.05, seed=2, churn=False, slots=1))
 
 
 def test_delta_variants():
-    run_both(scenarios.byzantine_injectors(2000, 12, 3, 0.05, delta=0, seed=2, churn=False, slots=1))
-    run_both(scenarios.byzantine_injectors(2000, 12, 3, 0.05, delta=5, seed=2))
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(2000, 12, 3, 0.05, delta=0, seed=2, churn=False, slots=1))
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(2000, 12, 3, 0.05, delta=5, seed=2))
 
 
 def test_injectors_and_user_events_together():
@@ -54,12 +39,10 @@ def test_injectors_and_user_events_together():
     ue = scenarios.user_event_storm(2500, 16, 4, seed=6, n_events=3)
     sc.user_events = ue.user_events
     sc.ops += [op for op in ue.ops if (op[0], op[2]) not in {(o[0], o[2]) for o in sc.ops}]
-    g, o = run_both(sc)
-    assert g.user_event_stats() == o.user_event_stats()
-    assert (g.user_event_records() == o.user_event_records()).all()
+    P.run_against_oracle(emu_sim, sc)
 
 
 @pytest.mark.parametrize("pp", [6, 15])
 def test_injectors_with_push_pull_rounds(pp):
     """Verdicts of a tick are taken before that tick's push-pull round, on the device as in the oracle."""
-    run_both(scenarios.byzantine_injectors(2500, 12, 3, 0.05, seed=5), push_pull_interval_ticks=pp)
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(2500, 12, 3, 0.05, seed=5), push_pull_interval_ticks=pp)

@@ -6,9 +6,9 @@ import ctypes as C
 import pytest
 
 import envelope_lib as E
-from emu_lib import lib
+import parity_lib as P
+from emu_lib import emu_sim, lib
 from serf_b200.sim import random_regular_graph
-from test_emu_parity import run_both
 
 
 @pytest.mark.parametrize("dedup", ["1", "0"])
@@ -18,7 +18,7 @@ def test_dedup_parity_and_probe(monkeypatch, dedup):
     L.emu_probe.restype = C.c_ulong
     L.emu_probe_reset()
     n = 12_000
-    run_both(E.leave_study(n, random_regular_graph(n, 16, 3), fanout=4, max_ticks=80))
-    run_both(E.crash_study(n, random_regular_graph(n, 12, 4), fanout=4))
+    P.run_against_oracle(emu_sim, E.leave_study(n, random_regular_graph(n, 16, 3), fanout=4, max_ticks=80))
+    P.run_against_oracle(emu_sim, E.crash_study(n, random_regular_graph(n, 12, 4), fanout=4))
     skipped = L.emu_probe(22)
     assert (skipped > 0) == (dedup == "1"), skipped

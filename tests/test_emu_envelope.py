@@ -10,28 +10,16 @@ import numpy as np
 import pytest
 
 import envelope_lib as E
+import parity_lib as P
 from emu_lib import emu_sim, lib
-from oracle_lib import oracle_sim
 from serf_b200 import SerfsimError
 from serf_b200.sim import random_regular_graph
-from test_emu_multi import check as check_sharded
-from test_emu_parity import assert_same, run_both
 
 
 def probes():
     L = lib()
     L.emu_probe.restype = C.c_ulong
     return L
-
-
-def production(sc, **cfg):
-    """Oracle (trace = 1) and the host build in production mode (trace = 0); both must agree."""
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    f = sc.build(emu_sim, trace=0, **cfg)
-    assert f.run_until_converged(sc.max_ticks) == to, sc.name
-    assert_same(f, o, sc.slots, with_hash=False)
-    return f, o
 
 
 # ---- irregular CSR -------------------------------------------------------------------------------------------
@@ -55,31 +43,30 @@ def test_irregular_leave_and_lan_crash_multi_tile():
     n = 12_000
     topo = E.irregular_graph(n, 3)
     assert np.diff(topo[0].astype(np.int64)).min() == 0
-    run_both(E.leave_study(n, topo, fanout=4, max_ticks=80))
+    P.run_against_oracle(emu_sim, E.leave_study(n, topo, fanout=4, max_ticks=80))
     L.emu_probe_reset()
-    production(E.leave_study(n, topo, fanout=3, seed=5, max_ticks=80))
-    production(E.crash_study(n, random_regular_graph(n, 12, 4), fanout=4))
+    P.run_against_oracle(emu_sim, E.leave_study(n, topo, fanout=3, seed=5, max_ticks=80), traces=(0,))
+    P.run_against_oracle(emu_sim, E.crash_study(n, random_regular_graph(n, 12, 4), fanout=4), traces=(0,))
     assert L.emu_probe(0) > 0 and L.emu_probe(1) > 0 and L.emu_probe(2) > 0, [L.emu_probe(i) for i in range(3)]
     assert L.emu_probe(4) > 0 and L.emu_probe(20) > 0, (L.emu_probe(4), L.emu_probe(20))
 
 
 def test_irregular_crash_short_timers_self_loops_duplicates():
     topo = E.irregular_graph(6000, 4, self_loops=0.05, duplicates=0.05)
-    run_both(E.crash_study(6000, topo, fanout=3, short_timers=True, max_ticks=120))
+    P.run_against_oracle(emu_sim, E.crash_study(6000, topo, fanout=3, short_timers=True, max_ticks=120))
 
 
 @pytest.mark.parametrize("seed", range(12))
 def test_irregular_fuzz(seed):
-    run_both(E.envelope_fuzz(seed, topology="irregular"))
+    P.run_against_oracle(emu_sim, E.envelope_fuzz(seed, topology="irregular"))
 
 
 def test_uniform_graph_general_path(monkeypatch):
     """SERFSIM_UDEG=0: a uniform graph through the general (row_ptr) path gives what the arithmetic row offsets give."""
     sc = E.leave_study(8000, random_regular_graph(8000, 12, 9), fanout=4)
-    a, o = production(sc)
+    a = P.run_against_oracle(emu_sim, sc, traces=(0,))
     monkeypatch.setenv("SERFSIM_UDEG", "0")
-    b, _ = production(sc)
-    assert (b.tick_trace() == a.tick_trace()).all() and b.state_hash() == a.state_hash()
+    P.assert_same(P.run_against_oracle(emu_sim, sc, traces=(0,)), a, with_hash=True)
 
 
 # ---- fan-out 6–8 × slots 9–16 --------------------------------------------------------------------------------
@@ -101,7 +88,7 @@ def test_fanout8_slots12_storm(sv, monkeypatch):
     monkeypatch.setenv("SERFSIM_SV", sv)
     L.emu_probe_reset()
     sc = E.crash_and_leave_study(3000, random_regular_graph(3000, 12, 7), fanout=8, slots=12)
-    run_both(sc)
+    P.run_against_oracle(emu_sim, sc)
     assert (L.emu_probe(21) > 20) == (sv == "1"), L.emu_probe(21)
 
 
@@ -109,7 +96,7 @@ def test_fanout8_slots12_storm(sv, monkeypatch):
 def test_wide_fuzz(seed):
     sc = E.envelope_fuzz(seed)
     assert sc.cfg["fanout"] >= 6 and sc.slots >= 9
-    run_both(sc)
+    P.run_against_oracle(emu_sim, sc)
 
 
 def test_fuzz_draws_the_whole_range():
@@ -124,16 +111,11 @@ def test_fuzz_draws_the_whole_range():
 def test_scheduler_switches_change_nothing(switches, monkeypatch):
     """DESIGN §5: skipping idle tiles / ticks and jumping over sleeping stretches changes no row, record or clock."""
     scs = [E.crash_study(5000, random_regular_graph(5000, 12, 8), fanout=4)] + [E.envelope_fuzz(s) for s in range(4)]
-    base = []
-    for sc in scs:
-        f, _ = production(sc)
-        base.append((f.tick_trace(), f.state_hash(), [f.records(s) for s in range(sc.slots)]))
+    base = [P.run_against_oracle(emu_sim, sc, traces=(0,)) for sc in scs]
     for k in switches:
         monkeypatch.setenv(k, "1")
-    for sc, (tr, h, recs) in zip(scs, base):
-        f, _ = production(sc)
-        assert (f.tick_trace() == tr).all() and f.state_hash() == h
-        assert all((f.records(s) == recs[s]).all() for s in range(sc.slots))
+    for sc, out in zip(scs, base):
+        P.assert_same(P.run_against_oracle(emu_sim, sc, traces=(0,)), out, with_hash=True, what=sc.name)
 
 
 # ---- sharded: shards that do and do not have a uniform degree ---------------------------------------------------
@@ -165,7 +147,7 @@ def test_sharded_mixed_uniform_and_irregular_shards(world):
     assert (deg[:shard] == 8).all() and np.unique(deg[shard:2 * shard]).size > 2
     sc = Scenario(f"mixed_{world}", n, 2, (rp, col), [3, shard + 7], [(0, Op.LEAVE, 3, 0), (0, Op.FAIL, shard + 7, 0)],
                   dict(fanout=4, seed=3, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2), max_ticks=120)
-    check_sharded(sc, world)
+    P.run_against_oracle(emu_sim, sc, world=world)
 
 
 # ---- ABI limits --------------------------------------------------------------------------------------------------
@@ -206,4 +188,4 @@ def test_fanout8_slots16_accepted_and_exact():
     ops = [(0, Op.LEAVE, int(s), 0) for s in subjects[:8]] + [(1, Op.FAIL, int(s), 0) for s in subjects[8:]]
     sc = Scenario("f8_r16", n, 16, E.irregular_graph(n, 5, hubs=1), subjects, ops,
                   dict(fanout=8, seed=9, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=1), max_ticks=150)
-    run_both(sc)
+    P.run_against_oracle(emu_sim, sc)

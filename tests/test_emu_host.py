@@ -6,33 +6,34 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import parity_lib as P
 from emu_lib import emu_sim, lib
 from oracle_lib import oracle_sim
 from serf_b200 import MemberStatus, scenarios
 from serf_b200.sim import Config, Op, SerfsimError
-from test_emu_parity import assert_same
 
 
 def test_step_by_step_equals_run_until_converged():
     sc = scenarios.random_graph_leave(2000, 12, 3, seed=2, slots=2)
     o = sc.build(oracle_sim, trace=1)
     to, ok = o.run_until_converged(sc.max_ticks)
+    ref = P.outputs(o, sc, None)
     g = sc.build(emu_sim, trace=1)
     for _ in range(to + 1):
         g.step(1)
-    assert_same(g, o, sc.slots)
+    P.assert_same(P.outputs(g, sc, None), ref, with_hash=True)
     h = sc.build(emu_sim, trace=0)
     h.step(5)
     h.step(to + 1 - 5)
-    assert_same(h, o, sc.slots, with_hash=False)
+    P.assert_same(P.outputs(h, sc, None), ref, with_hash=False)
 
 
 def test_max_ticks_reached_returns_not_converged():
     sc = scenarios.random_graph_leave(2000, 12, 3, seed=2)
     g, o = sc.build(emu_sim, trace=1), sc.build(oracle_sim, trace=1)
     assert g.run_until_converged(6) == o.run_until_converged(6) == (6, False)
-    assert g.run_until_converged(sc.max_ticks) == o.run_until_converged(sc.max_ticks)      # and both continue from there
-    assert_same(g, o, sc.slots)
+    tg, to = g.run_until_converged(sc.max_ticks), o.run_until_converged(sc.max_ticks)      # and both continue from there
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=True)
 
 
 def test_long_run_grows_the_trace_buffer():
@@ -42,21 +43,20 @@ def test_long_run_grows_the_trace_buffer():
     g.run_until_converged(sc.max_ticks), o.run_until_converged(sc.max_ticks)
     g.inject(1500, Op.JOIN, int(sc.subjects[0]), 0)
     o.inject(1500, Op.JOIN, int(sc.subjects[0]), 0)
-    assert g.run_until_converged(4000) == o.run_until_converged(4000)
+    tg, to = g.run_until_converged(4000), o.run_until_converged(4000)
     assert g.stats()["tick"] > 1500
-    assert_same(g, o, sc.slots)
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=True)
 
 
 def test_speculative_pipeline_gives_the_same_result(monkeypatch):
     sc = scenarios.random_graph_leave(3000, 12, 4, seed=3)
     o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
+    ref = P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
     monkeypatch.setenv("SERFSIM_SPECULATE", "1")
     for chunk in ("1", "4", "16"):
         monkeypatch.setenv("SERFSIM_CHUNK", chunk)
         g = sc.build(emu_sim, trace=0)
-        assert g.run_until_converged(sc.max_ticks) == to
-        assert_same(g, o, sc.slots, with_hash=False)
+        P.assert_same(P.outputs(g, sc, g.run_until_converged(sc.max_ticks)), ref, with_hash=False, what=f"chunk {chunk}")
     g = sc.build(emu_sim, trace=0)
     assert g.run_until_converged(7) == (7, False)
 
@@ -64,12 +64,7 @@ def test_speculative_pipeline_gives_the_same_result(monkeypatch):
 @pytest.mark.parametrize("chunk", ["1", "3", "9"])
 def test_chunk_size_does_not_change_results(monkeypatch, chunk):
     monkeypatch.setenv("SERFSIM_CHUNK", chunk)
-    sc = scenarios.fuzz(11)                                # has reaper / push-pull boundary ticks
-    o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
-    g = sc.build(emu_sim, trace=0)
-    assert g.run_until_converged(sc.max_ticks) == to
-    assert_same(g, o, sc.slots, with_hash=False)
+    P.run_against_oracle(emu_sim, scenarios.fuzz(11), traces=(0,))                # has reaper / push-pull boundary ticks
 
 
 def test_event_callback_reports_agreed_status_changes():
@@ -172,14 +167,14 @@ def test_multi_phase_production_mode_rewind(monkeypatch, seed, chunk):
     assert g.run_until_converged(sc.max_ticks) == o.run_until_converged(sc.max_ticks)
     for sim in (g, o):
         sim.inject(sim.stats()["tick"], Op.FAIL, int(sc.subjects[1]), 0)
-    assert g.run_until_converged(5000) == o.run_until_converged(5000)
-    assert_same(g, o, sc.slots, with_hash=False)
+    tg, to = g.run_until_converged(5000), o.run_until_converged(5000)
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=False)
     for sim in (g, o):                                               # and once more: the subject returns, a force-leave follows later
         t = sim.stats()["tick"]
         sim.inject(t, Op.REJOIN, int(sc.subjects[1]), 0)
         sim.inject(t + 3, Op.FORCE_LEAVE, 7, 0)
-    assert g.run_until_converged(5000) == o.run_until_converged(5000)
-    assert_same(g, o, sc.slots, with_hash=False)
+    tg, to = g.run_until_converged(5000), o.run_until_converged(5000)
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=False)
 
 
 def test_results_async_returns_the_getters_values():
@@ -228,12 +223,11 @@ def test_late_operations_in_sleeping_stretches(seed, monkeypatch):
     spec.loader.exec_module(gen)
     sc = gen.late(seed)
     o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
+    ref = P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
     for trace, chunk in ((0, None), (1, None), (0, str(2 + seed % 11))):
         if chunk:
             monkeypatch.setenv("SERFSIM_CHUNK", chunk)
         else:
             monkeypatch.delenv("SERFSIM_CHUNK", raising=False)
         g = sc.build(emu_sim, trace=trace)
-        assert g.run_until_converged(sc.max_ticks) == to
-        assert_same(g, o, sc.slots, with_hash=bool(trace))
+        P.assert_same(P.outputs(g, sc, g.run_until_converged(sc.max_ticks)), ref, with_hash=bool(trace), what=f"trace={trace} chunk={chunk}")

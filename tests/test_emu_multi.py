@@ -2,109 +2,25 @@
 host-compiled kernels (tests/emu); the "NVLink windows" are plain shared memory with real acquire/release on the
 flags, the host collectives (barrier, u64 all-reduce) are thread primitives.  Concatenated records and the
 all-reduced trace must equal the single oracle's — the comparisons of tests/test_gpu_multi.py at small sizes."""
-import threading
-
-import numpy as np
 import pytest
 
+import parity_lib as P
 from emu_lib import emu_sim
-from oracle_lib import oracle_sim
 from serf_b200 import scenarios
-
-
-class ThreadComm:
-    def __init__(self, world):
-        self.world = world
-        self.bar = threading.Barrier(world)
-        self.blobs = [None] * world
-        self.acc = None
-        self.lock = threading.Lock()
-
-    def hooks(self, rank):
-        def all_gather_bytes(b):
-            self.blobs[rank] = b
-            self.bar.wait()
-            out = list(self.blobs)
-            self.bar.wait()
-            return out
-
-        def barrier():
-            self.bar.wait()
-
-        def allreduce_u64(arr):
-            with self.lock:
-                if self.acc is None:
-                    self.acc = arr.copy()
-                else:
-                    self.acc = self.acc + arr                       # u64 wrap-around sum
-            self.bar.wait()
-            arr[:] = self.acc
-            self.bar.wait()
-            if rank == 0:
-                self.acc = None
-            self.bar.wait()
-        return all_gather_bytes, barrier, allreduce_u64
-
-
-def run_sharded(sc, world, trace=1, **cfg):
-    comm = ThreadComm(world)
-    res, errs = [None] * world, []
-
-    def worker(rank):
-        try:
-            g = sc.build(emu_sim, rank=rank, world_size=world, trace=trace, **cfg)
-            g.connect(*comm.hooks(rank))
-            ticks, ok = g.run_until_converged(sc.max_ticks)
-            res[rank] = dict(ticks=ticks, ok=ok, trace=g.tick_trace(), hash=g.state_hash(), clock=g.lamport_time(),
-                             rec=[g.records(s) for s in range(sc.slots)], first=g.first, count=g.count)
-            comm.bar.wait()
-        except BaseException as e:                                  # noqa: BLE001 — surface it in the main thread
-            errs.append(e)
-            comm.bar.abort()
-    th = [threading.Thread(target=worker, args=(r,)) for r in range(world)]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join(600)
-    if errs:
-        raise errs[0]
-    return res
-
-
-def check(sc, world, **cfg):
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to, oko = o.run_until_converged(sc.max_ticks)
-    n = o.stats()["tick"]
-    tro = o.tick_trace(0, n)
-    for trace in (1, 0):
-        res = run_sharded(sc, world, trace=trace, **cfg)
-        for r in res:
-            assert (r["ticks"], r["ok"]) == (to, oko)
-            for f in tro.dtype.names:                               # every rank holds the all-reduced (global) trace
-                if f == "hash" and not trace:
-                    continue
-                bad = np.nonzero(r["trace"][f] != tro[f])[0]
-                assert bad.size == 0, f"world {world} trace={trace}: field {f} first differs at tick {bad[0]}"
-            assert r["hash"] == o.state_hash()
-        assert (np.concatenate([r["clock"] for r in res]) == o.lamport_time()).all()
-        for s in range(sc.slots):
-            got = np.concatenate([r["rec"][s] for r in res])
-            bad = np.nonzero(got != o.records(s))[0]
-            assert bad.size == 0, f"world {world} trace={trace} slot {s}: record of node {bad[0]} differs"
 
 
 @pytest.mark.parametrize("world", [2, 3, 4])
 def test_sharded_random_graph(world):
-    check(scenarios.random_graph_leave(3001, 12, 3, seed=2, slots=1), world)
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(3001, 12, 3, seed=2, slots=1), world=world)
 
 
 @pytest.mark.parametrize("world", [2, 4])
 def test_sharded_multi_slot_fanout4(world):
-    check(scenarios.random_graph_leave(2500, 12, 4, seed=3, slots=3), world)
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(2500, 12, 4, seed=3, slots=3), world=world)
 
 
 def test_sharded_failure_detection():
-    check(scenarios.random_graph_fail(2000, 16, 3, seed=2), 2, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
+    P.run_against_oracle(emu_sim, scenarios.random_graph_fail(2000, 16, 3, seed=2), world=2, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
 
 
 @pytest.mark.parametrize("world", [2, 3])
@@ -118,83 +34,23 @@ def test_sharded_cluster_sleeps_through_the_suspicion_timers(world, monkeypatch)
     L.emu_probe.restype = C.c_ulong
     L.emu_probe_reset()
     monkeypatch.setenv("SERFSIM_CHUNK", "4")
-    check(scenarios.dissemination_storm(3000, 12, 3, slots=2, seed=3, with_fail=True), world)
+    P.run_against_oracle(emu_sim, scenarios.dissemination_storm(3000, 12, 3, slots=2, seed=3, with_fail=True), world=world)
     assert L.emu_probe(17) > 20 * world            # both trace modes, every rank
 
 
 @pytest.mark.parametrize("seed", [7, 9, 12])
 def test_sharded_fuzz(seed):
-    check(scenarios.fuzz(seed, n=600, slots=4), 2, push_pull_interval_ticks=0)
+    P.run_against_oracle(emu_sim, scenarios.fuzz(seed, n=600, slots=4), world=2, push_pull_interval_ticks=0)
 
 
 # ---- user events across shards: remote targets get kind-3 window entries (event bit + the origin's Lamport time) ----
-def run_sharded_events(sc, world, trace=1, **cfg):
-    comm = ThreadComm(world)
-    res, errs = [None] * world, []
-    E = len(sc.user_events)
-
-    def worker(rank):
-        try:
-            g = sc.build(emu_sim, rank=rank, world_size=world, trace=trace, **cfg)
-            g.connect(*comm.hooks(rank))
-            ticks, ok = g.run_until_converged(sc.max_ticks)
-            res[rank] = dict(ticks=ticks, ok=ok, trace=g.tick_trace(), hash=g.state_hash(), clock=g.lamport_time(),
-                             rec=[g.records(s) for s in range(sc.slots)], ue=g.user_event_records(), ue_stats=g.user_event_stats(),
-                             ltime=[g.user_event_ltime(e) for e in range(E)], seen=[g.user_event_seen(e) for e in range(E)],
-                             etime=g.event_time())
-            comm.bar.wait()
-        except BaseException as e:                                  # noqa: BLE001
-            errs.append(e)
-            comm.bar.abort()
-    th = [threading.Thread(target=worker, args=(r,)) for r in range(world)]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join(600)
-    if errs:
-        raise errs[0]
-    return res
-
-
-def check_events(sc, world, **cfg):
-    E = len(sc.user_events)
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to, oko = o.run_until_converged(sc.max_ticks)
-    n = o.stats()["tick"]
-    tro = o.tick_trace(0, n)
-    so = o.user_event_stats()
-    for trace in (1, 0):
-        res = run_sharded_events(sc, world, trace=trace, **cfg)
-        for r in res:
-            assert (r["ticks"], r["ok"]) == (to, oko)
-            for f in tro.dtype.names:
-                if f == "hash" and not trace:
-                    continue
-                bad = np.nonzero(r["trace"][f] != tro[f])[0]
-                assert bad.size == 0, f"world {world} trace={trace}: field {f} first differs at tick {bad[0]}"
-            assert r["hash"] == o.state_hash()
-            assert r["ltime"] == [o.user_event_ltime(e) for e in range(E)]
-            st = dict(r["ue_stats"])
-            st.pop("event_time")                                    # a maximum: shard-local by contract
-            assert st == {k: v for k, v in so.items() if k != "event_time"}
-        assert max(r["ue_stats"]["event_time"] for r in res) == so["event_time"]
-        got = np.concatenate([r["ue"] for r in res])
-        bad = np.nonzero(got != o.user_event_records())[0]
-        assert bad.size == 0, f"world {world} trace={trace}: event record of node {bad[0]} differs: {got[bad[0]]} vs {o.user_event_records()[bad[0]]}"
-        assert (np.concatenate([r["etime"] for r in res]) == o.event_time()).all()
-        for e in range(E):
-            assert (np.concatenate([r["seen"][e] for r in res]) == o.user_event_seen(e)).all()
-        for s in range(sc.slots):
-            assert (np.concatenate([r["rec"][s] for r in res]) == o.records(s)).all()
-
-
 @pytest.mark.parametrize("world", [2, 3])
 def test_sharded_user_events(world):
-    check_events(scenarios.user_event_storm(2501, 12, 3, seed=3, n_events=5, spacing=2, churn=30, with_leave=True), world)
+    P.run_against_oracle(emu_sim, scenarios.user_event_storm(2501, 12, 3, seed=3, n_events=5, spacing=2, churn=30, with_leave=True), world=world)
 
 
 def test_sharded_user_events_aliased_fanout4():
-    check_events(scenarios.user_event_storm(2000, 12, 4, seed=5, n_events=3, spacing=2, alias=True), 4)
+    P.run_against_oracle(emu_sim, scenarios.user_event_storm(2000, 12, 4, seed=5, n_events=3, spacing=2, alias=True), world=4)
 
 
 # ---- push-pull rounds across shards: partners on other ranks are read through the peer mapping of their snapshot ----
@@ -206,71 +62,28 @@ def test_sharded_push_pull(world, pp):
                             [(0, scenarios.Op.LEAVE, 3, 0), (1, scenarios.Op.FAIL, n // 2, 0), (40, scenarios.Op.REJOIN, n // 2, 0)],
                             dict(fanout=3, seed=4, retransmit_mult=1, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2),
                             max_ticks=3000)
-    check(sc, world, push_pull_interval_ticks=pp)
+    P.run_against_oracle(emu_sim, sc, world=world, push_pull_interval_ticks=pp)
 
 
 @pytest.mark.parametrize("seed", [3, 5, 11])
 def test_sharded_fuzz_with_push_pull_and_reaper(seed):
-    check(scenarios.fuzz(seed, n=500, slots=3), 2)
+    P.run_against_oracle(emu_sim, scenarios.fuzz(seed, n=500, slots=3), world=2)
 
 
 # ---- byzantine injectors across shards: triples in the peer's window, verdict by the receiving shard's drain kernel ----
-def check_byzantine(sc, world, **cfg):
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to, oko = o.run_until_converged(sc.max_ticks)
-    n = o.stats()["tick"]
-    tro = o.tick_trace(0, n)
-    for trace in (1, 0):
-        comm = ThreadComm(world)
-        res, errs = [None] * world, []
-
-        def worker(rank):
-            try:
-                g = sc.build(emu_sim, rank=rank, world_size=world, trace=trace, **cfg)
-                g.connect(*comm.hooks(rank))
-                ticks, ok = g.run_until_converged(sc.max_ticks)
-                res[rank] = dict(ticks=ticks, ok=ok, trace=g.tick_trace(), hash=g.state_hash(), flags=g.anomaly_flags(), stats=g.byzantine_stats(),
-                                 rec=[g.records(s) for s in range(sc.slots)], clock=g.lamport_time())
-                comm.bar.wait()
-            except BaseException as e:                              # noqa: BLE001
-                errs.append(e)
-                comm.bar.abort()
-        th = [threading.Thread(target=worker, args=(r,)) for r in range(world)]
-        for t in th:
-            t.start()
-        for t in th:
-            t.join(600)
-        if errs:
-            raise errs[0]
-        for r in res:
-            assert (r["ticks"], r["ok"]) == (to, oko)
-            for f in tro.dtype.names:
-                if f == "hash" and not trace:
-                    continue
-                bad = np.nonzero(r["trace"][f] != tro[f])[0]
-                assert bad.size == 0, f"world {world} trace={trace}: field {f} first differs at tick {bad[0]}"
-            assert r["hash"] == o.state_hash()
-            assert r["stats"] == o.byzantine_stats(), (r["stats"], o.byzantine_stats())
-        flags = np.concatenate([r["flags"] for r in res])
-        bad = np.nonzero(flags != o.anomaly_flags())[0]
-        assert bad.size == 0, f"world {world} trace={trace}: anomaly flag of node {bad[0]}"
-        for s in range(sc.slots):
-            assert (np.concatenate([r["rec"][s] for r in res]) == o.records(s)).all()
-
-
 @pytest.mark.parametrize("world", [2, 4])
 def test_sharded_byzantine(world):
-    check_byzantine(scenarios.byzantine_injectors(2400, 16, 4, 0.02, seed=1), world)
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(2400, 16, 4, 0.02, seed=1), world=world)
 
 
 def test_sharded_byzantine_heavy_three_ranks():
-    check_byzantine(scenarios.byzantine_injectors(1501, 12, 3, 0.2, seed=3), 3)
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(1501, 12, 3, 0.2, seed=3), world=3)
 
 
 def test_sharded_stage_overflow_path():
     """8 subjects × fan-out 8: a tile produces far more cross-shard entries than the shared-memory stage holds
     (3072 per CTA), so the write-through path behind the stage is taken — results unchanged."""
-    check(scenarios.random_graph_leave(1500, 12, 8, seed=6, slots=8), 2)
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(1500, 12, 8, seed=6, slots=8), world=2)
 
 
 def test_window_overflow_is_reported(monkeypatch):
@@ -279,7 +92,7 @@ def test_window_overflow_is_reported(monkeypatch):
     monkeypatch.setenv("SERFSIM_WIN_FACTOR", "0.0001")
     sc = scenarios.random_graph_leave(30000, 12, 8, seed=6, slots=8)
     with pytest.raises(SerfsimError) as ei:
-        run_sharded(sc, 2, trace=0)
+        P.run_ranks(sc, 2, 0)
     assert ei.value.code == -6
 
 
@@ -291,70 +104,23 @@ def test_sharded_fuzz_with_user_events_and_injectors(seed):
     sc = scenarios.fuzz_features(seed, n=(400 + 37 * seed) if seed < 100 else 300 + 13 * (seed % 40), slots=3 if seed < 100 else 1 + seed % 4)
     sc.max_ticks = 400 if seed < 100 else 300   # some injector runs never go quiet (reaper ticks keep merging): both sides stop at the cap
     world = (2 + seed % 2) if seed < 100 else 2 + seed % 3
-    o = sc.build(oracle_sim, trace=1)
-    to, oko = o.run_until_converged(sc.max_ticks)
-    n = o.stats()["tick"]
-    tro = o.tick_trace(0, n)
-    for trace in (1, 0):
-        comm = ThreadComm(world)
-        res, errs = [None] * world, []
-
-        def worker(rank):
-            try:
-                g = sc.build(emu_sim, rank=rank, world_size=world, trace=trace)
-                g.connect(*comm.hooks(rank))
-                ticks, ok = g.run_until_converged(sc.max_ticks)
-                r = dict(ticks=ticks, ok=ok, trace=g.tick_trace(), hash=g.state_hash(), rec=[g.records(s) for s in range(sc.slots)])
-                if sc.user_events is not None:
-                    r["ue"], r["ue_stats"] = g.user_event_records(), g.user_event_stats()
-                if sc.byzantine is not None:
-                    r["flags"], r["byz_stats"] = g.anomaly_flags(), g.byzantine_stats()
-                res[rank] = r
-                comm.bar.wait()
-            except BaseException as e:                              # noqa: BLE001
-                errs.append(e)
-                comm.bar.abort()
-        th = [threading.Thread(target=worker, args=(r,)) for r in range(world)]
-        for t in th:
-            t.start()
-        for t in th:
-            t.join(600)
-        if errs:
-            raise errs[0]
-        for r in res:
-            assert (r["ticks"], r["ok"]) == (to, oko)
-            for f in tro.dtype.names:
-                if f == "hash" and not trace:
-                    continue
-                assert (r["trace"][f] == tro[f]).all(), f
-            assert r["hash"] == o.state_hash()
-        for s in range(sc.slots):
-            assert (np.concatenate([r["rec"][s] for r in res]) == o.records(s)).all()
-        if sc.user_events is not None:
-            assert (np.concatenate([r["ue"] for r in res]) == o.user_event_records()).all()
-            so = o.user_event_stats()
-            for r in res:
-                assert {k: v for k, v in r["ue_stats"].items() if k != "event_time"} == {k: v for k, v in so.items() if k != "event_time"}
-        if sc.byzantine is not None:
-            assert (np.concatenate([r["flags"] for r in res]) == o.anomaly_flags()).all()
-            assert all(r["byz_stats"] == o.byzantine_stats() for r in res)
+    P.run_against_oracle(emu_sim, sc, world=world)
 
 
 def test_sharded_user_events_need_bigger_windows():
     """5 events × fan-out 3 from every node: more cross-shard entries per tick than the windows serfsim_create sizes for
     membership traffic alone — serfsim_set_user_events must have resized them (it used to overflow at this size)."""
-    check_events(scenarios.user_event_storm(20_000, 16, 3, seed=3, n_events=5, spacing=2, churn=50, with_leave=True), 2)
+    P.run_against_oracle(emu_sim, scenarios.user_event_storm(20_000, 16, 3, seed=3, n_events=5, spacing=2, churn=50, with_leave=True), world=2)
 
 
 @pytest.mark.parametrize("world", [2, 3])
 def test_sharded_user_events_with_push_pull(world):
     """Event replay of a push-pull round when the partner lives in another shard (its event snapshot is peer-mapped)."""
-    check_events(scenarios.user_event_storm(2001, 8, 2, seed=6, n_events=5, spacing=2, churn=30, with_leave=True), world,
-                 push_pull_interval_ticks=5, retransmit_mult=1)
+    P.run_against_oracle(emu_sim, scenarios.user_event_storm(2001, 8, 2, seed=6, n_events=5, spacing=2, churn=30, with_leave=True), world=world, push_pull_interval_ticks=5, retransmit_mult=1)
 
 
 def test_sharded_byzantine_with_push_pull():
-    check_byzantine(scenarios.byzantine_injectors(2400, 12, 3, 0.05, seed=5), 3, push_pull_interval_ticks=6)
+    P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(2400, 12, 3, 0.05, seed=5), world=3, push_pull_interval_ticks=6)
 
 
 def test_loopback_profiling_aid_runs():

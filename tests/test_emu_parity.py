@@ -6,79 +6,44 @@ PTX-level behaviour); it catches indexing / control-flow / host-logic mistakes b
 import numpy as np
 import pytest
 
+import parity_lib as P
 from emu_lib import emu_sim
 from oracle_lib import oracle_sim
 from serf_b200 import MemberStatus, scenarios
 
 
-def assert_same(g, o, slots, with_hash=True):
-    sg, so = g.stats(), o.stats()
-    assert sg == so, (sg, so)
-    n = sg["tick"]
-    tg, to = g.tick_trace(0, n), o.tick_trace(0, n)
-    for f in tg.dtype.names:
-        if f == "hash" and not with_hash:
-            continue
-        bad = np.nonzero(tg[f] != to[f])[0]
-        assert bad.size == 0, f"trace field {f} first differs at tick {bad[0]}: emu {tg[f][bad[0]]} oracle {to[f][bad[0]]}"
-    assert (g.lamport_time() == o.lamport_time()).all()
-    assert (g.lamport_time_u32() == o.lamport_time()).all()
-    for s in range(slots):
-        rg, ro = g.records(s), o.records(s)
-        bad = np.nonzero(rg != ro)[0]
-        assert bad.size == 0, f"slot {s}: record of node {bad[0]} differs: emu {rg[bad[0]]} oracle {ro[bad[0]]}"
-        assert (g.member_status(s) == o.member_status(s)).all()
-        assert (g.status_ltime(s) == o.status_ltime(s)).all()
-        assert (g.status_ltime_u32(s) == o.status_ltime(s)).all()                 # compact getters: same values, half the bytes
-        assert (g.incarnation(s) == o.incarnation(s)).all()
-        assert (g.ml_state(s) == o.ml_state(s)).all()
-    assert g.state_hash() == o.state_hash()
-
-
-def run_both(sc, **cfg):
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    g = sc.build(emu_sim, trace=1, **cfg)
-    assert g.run_until_converged(sc.max_ticks) == to
-    assert_same(g, o, sc.slots)
-    f = sc.build(emu_sim, trace=0, **cfg)                 # production mode: tile skipping, lazy loads, no per-tick hash
-    assert f.run_until_converged(sc.max_ticks) == to
-    assert_same(f, o, sc.slots, with_hash=False)
-    return g, o
-
-
 @pytest.mark.parametrize("seed", [1, 2])
 def test_config0_full_mesh_256(seed):
-    g, o = run_both(scenarios.full_mesh_leave(256, 3, seed))
-    assert (g.member_status(0)[1:] == MemberStatus.LEFT).all()
+    out = P.run_against_oracle(emu_sim, scenarios.full_mesh_leave(256, 3, seed))
+    assert (out["member_status"][0][1:] == MemberStatus.LEFT).all()
 
 
 def test_random_graph_single_slot():
-    run_both(scenarios.random_graph_leave(6000, 16, 3, seed=1))
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(6000, 16, 3, seed=1))
 
 
 def test_random_graph_multi_slot_fanout4():
-    run_both(scenarios.random_graph_leave(3000, 12, 4, seed=5, slots=4))
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(3000, 12, 4, seed=5, slots=4))
 
 
 def test_fanout_eight():
-    run_both(scenarios.random_graph_leave(2000, 12, 8, seed=3, slots=2))
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(2000, 12, 8, seed=3, slots=2))
 
 
 def test_failure_detection():
     sc = scenarios.random_graph_fail(2500, 16, 3, seed=2)
-    g, o = run_both(sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
-    assert (np.delete(g.member_status(0), 5) == MemberStatus.FAILED).all()
+    out = P.run_against_oracle(emu_sim, sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
+    assert (np.delete(out["member_status"][0], 5) == MemberStatus.FAILED).all()
 
 
 def test_small_world_churn():
     sc = scenarios.small_world_churn(3000, 12, 0.1, 0.05, slots=4, window=30, seed=3)
-    run_both(sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
+    P.run_against_oracle(emu_sim, sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
 
 
 @pytest.mark.parametrize("seed", range(40))
 def test_fuzz(seed):
-    run_both(scenarios.fuzz(seed))
+    P.run_against_oracle(emu_sim, scenarios.fuzz(seed))
 
 
 def test_compaction_path_is_taken_and_exact():
@@ -89,13 +54,8 @@ def test_compaction_path_is_taken_and_exact():
     L = lib()
     L.emu_probe.restype = C.c_ulong
     L.emu_probe_reset()
-    sc = scenarios.random_graph_leave(6000, 16, 3, seed=1)
-    o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
-    f = sc.build(emu_sim, trace=0)
-    assert f.run_until_converged(sc.max_ticks) == to
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(6000, 16, 3, seed=1), traces=(0,))
     assert L.emu_probe(0) > 0 and L.emu_probe(1) > 0 and L.emu_probe(2) > 0
-    assert_same(f, o, sc.slots, with_hash=False)
 
 
 def test_remove_failed_node_prune_reference_scenario():
@@ -103,16 +63,16 @@ def test_remove_failed_node_prune_reference_scenario():
     longer list the failed node (`wait_until_num_nodes(2, ..)` in the reference)."""
     for n in (3, 40):
         sc = scenarios.remove_failed_node_prune(n)
-        f, o = run_both(sc)
-        st = f.member_status(0)
+        out = P.run_against_oracle(emu_sim, sc)
+        st = out["member_status"][0]
         assert (np.delete(st, 1) == MemberStatus.NONE).all(), st          # erased from every survivor's member table
-        tr = o.tick_trace()
+        tr = out["trace"]
         assert tr["pending"][sc.ops[1][0] - 1] == 0                       # the failure had been detected and had settled before the prune
 
 
 @pytest.mark.parametrize("seed", range(24))
 def test_fuzz_prune(seed):
-    run_both(scenarios.fuzz_prune(seed))
+    P.run_against_oracle(emu_sim, scenarios.fuzz_prune(seed))
 
 
 def test_sleeping_views_timer_wheel_and_idle_ticks():
@@ -127,6 +87,7 @@ def test_sleeping_views_timer_wheel_and_idle_ticks():
     sc = scenarios.dissemination_storm(3000, 12, 3, slots=2, seed=3, with_fail=True)
     o = sc.build(oracle_sim, trace=1)
     to = o.run_until_converged(sc.max_ticks)
+    ref = P.outputs(o, sc, to)
     assert to[0] > 60
     import os
     for trace, chunk in ((0, None), (1, None), (0, "4"), (1, "5")):
@@ -135,7 +96,7 @@ def test_sleeping_views_timer_wheel_and_idle_ticks():
         if chunk:
             os.environ["SERFSIM_CHUNK"] = chunk            # small launch chunks: the host learns early that the cluster sleeps
         try:
-            assert f.run_until_converged(sc.max_ticks) == to
+            got = P.outputs(f, sc, f.run_until_converged(sc.max_ticks))
         finally:
             os.environ.pop("SERFSIM_CHUNK", None)
         # skipped on the device (launched before the host learnt that the cluster sleeps, probe 3) or not launched at all (probe 17)
@@ -145,14 +106,14 @@ def test_sleeping_views_timer_wheel_and_idle_ticks():
         if not trace:
             assert L.emu_probe(5) > 0
             assert L.emu_probe(20) > 0             # nodes of a due tile whose own deadline (node_due) lies later: no view visited
-        assert_same(f, o, sc.slots, with_hash=bool(trace))
+        P.assert_same(got, ref, with_hash=bool(trace), what=f"trace={trace} chunk={chunk}")
     # stepping one tick at a time takes the same decisions (the scheduler words live on the device, not in the call)
     f = sc.build(emu_sim, trace=1)
     for _ in range(to[0] + 1):
         f.step(1)
     o2 = sc.build(oracle_sim, trace=1)
     o2.step(to[0] + 1)
-    assert_same(f, o2, sc.slots)
+    P.assert_same(P.outputs(f, sc, None), P.outputs(o2, sc, None), with_hash=True)
 
 
 @pytest.mark.parametrize("ahead", ["0", "2"])
@@ -169,7 +130,7 @@ def test_multi_slot_requests_one_tile_ahead(ahead, monkeypatch):
     L.emu_probe_reset()
     for sc in (scenarios.dissemination_storm(3000, 12, 3, slots=2, seed=3, with_fail=True), scenarios.random_graph_leave(5000, 16, 4, seed=2, slots=3),
                scenarios.fuzz(3), scenarios.fuzz(11), scenarios.fuzz_prune(5)):
-        run_both(sc)
+        P.run_against_oracle(emu_sim, sc)
     if ahead == "2":
         assert L.emu_probe(19) > 1000 and L.emu_probe(18) > 100, (L.emu_probe(19), L.emu_probe(18))
     else:
@@ -191,11 +152,7 @@ def test_single_view_ticks(mode, monkeypatch):
     scs = [scenarios.dissemination_storm(3000, 12, 3, slots=2, seed=3, with_fail=True), scenarios.dissemination_storm(2500, 10, 4, slots=3, seed=5, with_fail=True)]
     scs += [scenarios.fuzz(k) for k in range(12)] + [scenarios.fuzz_prune(k) for k in range(6)]
     for sc in scs:
-        o = sc.build(oracle_sim, trace=1)
-        to = o.run_until_converged(sc.max_ticks)
-        f = sc.build(emu_sim, trace=0)
-        assert f.run_until_converged(sc.max_ticks) == to, sc.name
-        assert_same(f, o, sc.slots, with_hash=False)
+        P.run_against_oracle(emu_sim, sc, traces=(0,))
     if mode == "1":
         assert L.emu_probe(21) > 20, L.emu_probe(21)
     else:
@@ -205,33 +162,14 @@ def test_single_view_ticks(mode, monkeypatch):
 def test_config1_shape_100k_nodes():
     """BASELINE configs[1] at full size (100 K-node random graph, fan-out 3) through the host-compiled kernels:
     391 tiles over 4 CTAs, dense and sparse ticks, production mode (trace off)."""
-    sc = scenarios.random_graph_leave(100_000, 16, 3, seed=1)
-    o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
-    f = sc.build(emu_sim, trace=0)
-    assert f.run_until_converged(sc.max_ticks) == to
-    assert_same(f, o, sc.slots, with_hash=False)
+    P.run_against_oracle(emu_sim, scenarios.random_graph_leave(100_000, 16, 3, seed=1), traces=(0,))
 
 
 def test_config2_shape_small_world_churn_100k():
     """BASELINE configs[2] shape (small world, 5 % of the nodes crash / return, 8 tracked subjects, probing on) at
     100 K nodes, production mode."""
     sc = scenarios.small_world_churn(100_000, 16, 0.1, 0.05, slots=8, window=60, seed=3)
-    cfg = dict(suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    f = sc.build(emu_sim, trace=0, **cfg)
-    assert f.run_until_converged(sc.max_ticks) == to
-    assert_same(f, o, sc.slots, with_hash=False)
-
-
-def _feature_checks(g, o, sc):
-    if sc.user_events is not None:
-        assert g.user_event_stats() == o.user_event_stats()
-        assert (g.user_event_records() == o.user_event_records()).all()
-    if sc.byzantine is not None:
-        assert g.byzantine_stats() == o.byzantine_stats()
-        assert (g.anomaly_flags() == o.anomaly_flags()).all()
+    P.run_against_oracle(emu_sim, sc, traces=(0,), suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
 
 
 @pytest.mark.parametrize("seed", range(30))
@@ -239,13 +177,7 @@ def test_fuzz_with_user_events_and_injectors(seed):
     """Every operation kind, reaper, probing, tracked user events (with aliases) and byzantine injectors at once."""
     sc = scenarios.fuzz_features(seed)
     sc.max_ticks = 1200                    # injector runs with push-pull / reaper rounds may never go quiet: both sides stop at the cap
-    o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
-    for trace in (1, 0):
-        g = sc.build(emu_sim, trace=trace)
-        assert g.run_until_converged(sc.max_ticks) == to
-        assert_same(g, o, sc.slots, with_hash=bool(trace))
-        _feature_checks(g, o, sc)
+    P.run_against_oracle(emu_sim, sc)
 
 
 @pytest.mark.skipif(not __import__("os").environ.get("SERFSIM_SLOW"), reason="≈ 2 min and 3 GB: set SERFSIM_SLOW=1")
@@ -260,9 +192,4 @@ def test_bench_workload_full_10m_nodes():
     olib().oracle_sim_set_threads(o._h, 8)
     o.reset(sc.cfg["seed"])
     sc.schedule(o)
-    assert o.run_until_converged(sc.max_ticks) == tf
-    assert f.state_hash() == o.state_hash() and f.stats() == o.stats()
-    tr, to = f.tick_trace(), o.tick_trace()
-    for name in tr.dtype.names:
-        if name != "hash":
-            assert (tr[name] == to[name]).all(), name
+    P.assert_same(P.outputs(f, sc, tf), P.outputs(o, sc, o.run_until_converged(sc.max_ticks)), with_hash=False)

@@ -19,6 +19,7 @@ import functools
 import pytest
 
 import envelope_lib as E
+import parity_lib as P
 import scaled_fuzz_lib as S
 from emu_lib import emu_sim, lib
 from oracle_lib import oracle_sim
@@ -45,7 +46,7 @@ def _probes():
 def oracle_run(seed):
     sc = S.scaled_fuzz(seed, n=host_n(seed))
     o = sc.build(oracle_sim, trace=1)
-    return sc, S.oracle_outputs(o, sc, o.run_until_converged(sc.max_ticks))
+    return sc, P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
 
 
 @functools.lru_cache(None)
@@ -54,10 +55,9 @@ def production_run(seed):
     sc, ref = oracle_run(seed)
     L = _probes()
     L.emu_probe_reset()
-    f = sc.build(emu_sim, trace=0)
-    got = S.outputs(f, sc, f.run_until_converged(sc.max_ticks))
+    got = E.product_run(sc.build(emu_sim, trace=0), sc)
     probes = {i: int(L.emu_probe(i)) for i in PROBES}
-    S.assert_same_outputs(got, ref, sc, with_hash=False, what=f"{sc.name} trace=0")
+    P.assert_same(got["out"], ref, with_hash=False, what=f"{sc.name} trace=0")
     return got, probes
 
 
@@ -66,7 +66,7 @@ def test_scaled_fuzz(seed):
     sc, ref = oracle_run(seed)
     assert sc.n % E.TILE != 0 and sc.n >= 16 * E.TILE
     g = sc.build(emu_sim, trace=1)
-    S.assert_same_outputs(S.outputs(g, sc, g.run_until_converged(sc.max_ticks)), ref, sc, with_hash=True, what=f"{sc.name} trace=1")
+    P.assert_same(P.outputs(g, sc, g.run_until_converged(sc.max_ticks)), ref, with_hash=True, what=f"{sc.name} trace=1")
     production_run(seed)
 
 
@@ -96,6 +96,6 @@ def test_random_schedule_and_grid_change_nothing():
     seed = 2
     sc, ref = oracle_run(seed)
     got = E.run_isolated([dict(sc=sc, trace=0)], {"SERFSIM_GPU_TESTS_ON_EMU": "1", "SERFSIM_EMU_SCHED": "random:11", "SERFSIM_EMU_SMS": "3"})[0]
-    S.assert_same_outputs(got, ref, sc, with_hash=False, what=f"{sc.name} random schedule")
+    P.assert_same(got["out"], ref, with_hash=False, what=f"{sc.name} random schedule")
     base, _ = production_run(seed)
     assert (got["view_kinds"] == base["view_kinds"]).all()

@@ -1,63 +1,39 @@
 """User-event kernel logic on the CPU: uevent_kernel.cu (and the host code around it) compiled for the host by
 tests/emu, against the oracle's literal ring-buffer model — the comparisons of tests/test_gpu_z_uevent.py at sizes a
 fiber scheduler finishes in seconds."""
-import numpy as np
 import pytest
 
+import parity_lib as P
 from emu_lib import emu_sim
 from oracle_lib import oracle_sim
 from serf_b200 import scenarios
 from serf_b200.sim import SerfsimError
-from test_emu_parity import assert_same
-
-
-def assert_same_events(g, o, n_events):
-    rg, ro = g.user_event_records(), o.user_event_records()
-    bad = np.nonzero(rg != ro)[0]
-    assert bad.size == 0, f"event record of node {bad[0]} differs: emu {rg[bad[0]]} oracle {ro[bad[0]]}"
-    assert g.user_event_stats() == o.user_event_stats(), (g.user_event_stats(), o.user_event_stats())
-    assert (g.event_time() == o.event_time()).all()
-    for e in range(n_events):
-        assert g.user_event_ltime(e) == o.user_event_ltime(e)
-        assert (g.user_event_seen(e) == o.user_event_seen(e)).all()
-
-
-def run_both(sc, **cfg):
-    E = len(sc.user_events)
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    for trace in (1, 0):
-        g = sc.build(emu_sim, trace=trace, **cfg)
-        assert g.run_until_converged(sc.max_ticks) == to
-        assert_same(g, o, sc.slots, with_hash=bool(trace))
-        assert_same_events(g, o, E)
-    return g, o
 
 
 @pytest.mark.parametrize("seed", [1, 2])
 def test_user_event_storm(seed):
-    g, o = run_both(scenarios.user_event_storm(4000, 16, 3, seed=seed, n_events=4, spacing=3))
-    assert g.user_event_stats()["event_queue"] == 0
+    out = P.run_against_oracle(emu_sim, scenarios.user_event_storm(4000, 16, 3, seed=seed, n_events=4, spacing=3))
+    assert out["user_event_stats"]["event_queue"] == 0
 
 
 def test_user_events_with_churn_and_leave():
-    run_both(scenarios.user_event_storm(3000, 12, 3, seed=4, n_events=6, spacing=1, churn=60, with_leave=True))
+    P.run_against_oracle(emu_sim, scenarios.user_event_storm(3000, 12, 3, seed=4, n_events=6, spacing=1, churn=60, with_leave=True))
 
 
 def test_aliased_events():
-    g, o = run_both(scenarios.user_event_storm(2500, 12, 3, seed=5, n_events=3, spacing=2, alias=True))
-    assert ((g.user_event_seen(0) + g.user_event_seen(1)) == 1).all()
+    out = P.run_against_oracle(emu_sim, scenarios.user_event_storm(2500, 12, 3, seed=5, n_events=3, spacing=2, alias=True))
+    assert ((out["user_event_seen"][0] + out["user_event_seen"][1]) == 1).all()
 
 
 @pytest.mark.parametrize("fanout,events", [(1, 2), (4, 8), (8, 3)])
 def test_fanouts_and_event_counts(fanout, events):
-    run_both(scenarios.user_event_storm(1500, 10, fanout, seed=7, n_events=events, spacing=1, churn=20))
+    P.run_against_oracle(emu_sim, scenarios.user_event_storm(1500, 10, fanout, seed=7, n_events=events, spacing=1, churn=20))
 
 
 def test_user_events_with_failure_detection():
     sc = scenarios.user_event_storm(2500, 16, 3, seed=8, n_events=4, spacing=4)
     sc.ops.append((2, scenarios.Op.FAIL, 0, 0))
-    run_both(sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
+    P.run_against_oracle(emu_sim, sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
 
 
 def test_reset_clears_event_state():
@@ -88,8 +64,7 @@ def test_user_events_with_push_pull_rounds(pp):
     """retransmit_mult 1 leaves the gossip of the events incomplete; push-pull rounds replay the partner's event ring
     (delegate.rs:539-552) and witness its event clock until everybody has everything."""
     sc = scenarios.user_event_storm(2500, 8, 2, seed=6, n_events=5, spacing=2, churn=30, with_leave=True)
-    g, o = run_both(sc, push_pull_interval_ticks=pp, retransmit_mult=1)
-    st = o.user_event_stats()
+    st = P.run_against_oracle(emu_sim, sc, push_pull_interval_ticks=pp, retransmit_mult=1)["user_event_stats"]
     gossip_only = scenarios.user_event_storm(2500, 8, 2, seed=6, n_events=5, spacing=2, churn=30, with_leave=True).build(oracle_sim, trace=1, retransmit_mult=1)
     gossip_only.run_until_converged(sc.max_ticks)
     assert st["delivered"] > gossip_only.user_event_stats()["delivered"]        # the rounds did deliver events gossip had missed

@@ -2,11 +2,13 @@
 The id range is sharded over 2 (or 4) ranks, cross-shard gossip goes through the NVLink windows, and the
 concatenated records / summed trace must equal the CPU oracle's — i.e. the result is independent of the sharding."""
 import os
+import pickle
 import sys
 
-import numpy as np
 import pytest
 import torch
+
+import parity_lib as P
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,20 +24,11 @@ def _worker(rank, world, port, scen_args, outdir):
     from serf_b200 import dist as sdist
     name, kwargs, cfg = scen_args
     sc = getattr(scenarios, name)(**kwargs)
-    g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), device=rank, rank=rank, world_size=world, trace=1, **cfg)
+    g = sc.build(GossipSim, device=rank, rank=rank, world_size=world, trace=1, **cfg)
     sdist.connect(g, dist, torch.device("cuda", rank))
-    ticks, ok = g.run_until_converged(sc.max_ticks)
-    tr = g.tick_trace()
-    extra = {}
-    if sc.user_events is not None:                 # collective getters: every rank makes the same calls in the same order
-        st = g.user_event_stats()
-        extra.update(ue=g.user_event_records(), ue_stats=np.array([st[k] for k in sorted(st)], dtype=np.uint64),
-                     ue_ltime=np.array([g.user_event_ltime(e) for e in range(len(sc.user_events))], dtype=np.uint64))
-    if sc.byzantine is not None:
-        bz = g.byzantine_stats()
-        extra.update(flags=g.anomaly_flags(), byz_stats=np.array([bz[k] for k in sorted(bz)], dtype=np.uint64))
-    np.savez(os.path.join(outdir, f"r{rank}.npz"), ticks=ticks, ok=ok, trace=tr, first=g.first, count=g.count, hash=np.uint64(g.state_hash()),
-             clock=g.lamport_time(), **{f"rec{s}": g.records(s) for s in range(sc.slots)}, **extra)
+    out = P.outputs(g, sc, g.run_until_converged(sc.max_ticks))
+    with open(os.path.join(outdir, f"r{rank}.pkl"), "wb") as f:
+        pickle.dump(out, f)
     dist.barrier()
     dist.destroy_process_group()
 
@@ -50,7 +43,11 @@ def _run(world, scen_args, tmp_path):
     for p in procs:
         p.join(600)
         assert p.exitcode == 0
-    return [np.load(os.path.join(str(tmp_path), f"r{r}.npz")) for r in range(world)]
+    res = []
+    for r in range(world):
+        with open(os.path.join(str(tmp_path), f"r{r}.pkl"), "rb") as f:
+            res.append(pickle.load(f))
+    return res
 
 
 WORLDS = [int(x) for x in os.environ.get("SERFSIM_TEST_WORLDS", "2,4").split(",")]
@@ -73,35 +70,10 @@ WORLDS = [int(x) for x in os.environ.get("SERFSIM_TEST_WORLDS", "2,4").split(","
 def test_sharded_equals_oracle(world, scen, tmp_path):
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
     from oracle_lib import oracle_sim
     from serf_b200 import scenarios
     name, kwargs, cfg = scen
     sc = getattr(scenarios, name)(**kwargs)
     o = sc.build(oracle_sim, trace=1, **cfg)
-    to, oko = o.run_until_converged(sc.max_ticks)
-    res = _run(world, scen, tmp_path)
-    n = o.stats()["tick"]
-    tro = o.tick_trace(0, n)
-    for r in res:
-        assert (int(r["ticks"]), bool(r["ok"])) == (to, oko)
-        for f in tro.dtype.names:                       # every rank holds the all-reduced (global) trace
-            assert (r["trace"][f] == tro[f]).all(), f
-        assert int(r["hash"]) == o.state_hash()
-    assert (np.concatenate([r["clock"] for r in res]) == o.lamport_time()).all()
-    for s in range(sc.slots):
-        assert (np.concatenate([r[f"rec{s}"] for r in res]) == o.records(s)).all()
-    if sc.user_events is not None:
-        assert (np.concatenate([r["ue"] for r in res]) == o.user_event_records()).all()
-        so = o.user_event_stats()
-        keys = sorted(so)
-        for r in res:
-            got = dict(zip(keys, (int(x) for x in r["ue_stats"])))
-            assert {k: v for k, v in got.items() if k != "event_time"} == {k: v for k, v in so.items() if k != "event_time"}
-            assert [int(x) for x in r["ue_ltime"]] == [o.user_event_ltime(e) for e in range(len(sc.user_events))]
-        assert max(int(dict(zip(keys, r["ue_stats"]))["event_time"]) for r in res) == so["event_time"]
-    if sc.byzantine is not None:
-        assert (np.concatenate([r["flags"] for r in res]) == o.anomaly_flags()).all()
-        bo = o.byzantine_stats()
-        for r in res:
-            assert dict(zip(sorted(bo), (int(x) for x in r["byz_stats"]))) == bo
+    ref = P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
+    P.assert_same(P.merge_ranks(_run(world, scen, tmp_path)), ref, with_hash=True, what=f"world {world}")

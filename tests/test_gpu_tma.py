@@ -6,8 +6,8 @@ import os
 
 import pytest
 
-from serf_b200 import scenarios
-from test_gpu_parity import run_both
+import parity_lib as P
+from serf_b200 import GossipSim, scenarios
 
 pytestmark = pytest.mark.gpu
 
@@ -27,19 +27,19 @@ def _selected(capfd):
 
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_tma_config1_random_graph_100k(seed, capfd):
-    run_both(scenarios.random_graph_leave(100_000, 16, 3, seed))
+    P.run_against_oracle(GossipSim, scenarios.random_graph_leave(100_000, 16, 3, seed))
     assert _selected(capfd)
 
 
 def test_tma_fanout4_ragged_tail(capfd):
-    run_both(scenarios.random_graph_leave(60_001, 12, 4, seed=5))          # last tile partly filled
+    P.run_against_oracle(GossipSim, scenarios.random_graph_leave(60_001, 12, 4, seed=5))          # last tile partly filled
     assert _selected(capfd)
 
 
 def test_tma_failure_detection(capfd):
     sc = scenarios.random_graph_fail(20_000, 16, 3, seed=2)
     sc.slots, sc.subjects, sc.ops = 1, sc.subjects[:1], [op for op in sc.ops if op[2] == int(sc.subjects[0])]
-    run_both(sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
+    P.run_against_oracle(GossipSim, sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
     assert _selected(capfd)
 
 
@@ -47,5 +47,5 @@ def test_tma_failure_detection(capfd):
 def test_tma_fuzz_single_slot(seed, capfd):
     sc = scenarios.fuzz(seed, slots=1)
     sc.max_ticks = 1500
-    run_both(sc)
+    P.run_against_oracle(GossipSim, sc)
     assert _selected(capfd)

@@ -2,61 +2,34 @@
 bit for bit — anomaly flags, injector counters, and everything the honest parity tests compare (records, clocks, every
 trace row, state hash), with the per-tick hash on (trace = 1) and in production mode (trace = 0, tile skipping on).
 The model is defined by the oracle (no reference semantics, SURVEY §7.4)."""
-import numpy as np
 import pytest
 
-from oracle_lib import oracle_sim
-from serf_b200 import scenarios
-from test_gpu_parity import assert_same, gpu_sim
+import parity_lib as P
+from serf_b200 import GossipSim, scenarios
 
 pytestmark = pytest.mark.gpu
-
-
-def run_both(sc, **cfg):
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    for trace in (1, 0):
-        g = sc.build(gpu_sim, trace=trace, **cfg)
-        assert g.run_until_converged(sc.max_ticks) == to
-        if trace:
-            assert_same(g, o, sc.slots)
-        else:
-            n = o.stats()["tick"]
-            trg, tro = g.tick_trace(0, n), o.tick_trace(0, n)
-            for name in trg.dtype.names:
-                if name != "hash":
-                    bad = np.nonzero(trg[name] != tro[name])[0]
-                    assert bad.size == 0, f"trace=0: field {name} first differs at tick {bad[0]}"
-            assert g.state_hash() == o.state_hash() and g.stats() == o.stats()
-            for s in range(sc.slots):
-                assert (g.records(s) == o.records(s)).all()
-        fg, fo = g.anomaly_flags(), o.anomaly_flags()
-        bad = np.nonzero(fg != fo)[0]
-        assert bad.size == 0, f"anomaly flag of node {bad[0]}: gpu {fg[bad[0]]} oracle {fo[bad[0]]}"
-        assert g.byzantine_stats() == o.byzantine_stats()
-    return g, o
 
 
 @pytest.mark.parametrize("seed", [1, 2])
 def test_config4_shape_100k_one_percent(seed):
     sc = scenarios.byzantine_injectors(100_000, 16, 4, 0.01, seed=seed)
-    g, o = run_both(sc)
-    assert g.anomaly_flags()[sc.byzantine].mean() > 0.95
+    out = P.run_against_oracle(GossipSim, sc)
+    assert out["anomaly_flags"][sc.byzantine].mean() > 0.95
 
 
 def test_heavy_injection_changes_the_trace():
     """20 % injectors: stale copies are accepted by lagging nodes and re-gossiped, so the honest trace itself differs
     from the injector-free run — and must still match the oracle."""
-    run_both(scenarios.byzantine_injectors(30_000, 16, 4, 0.2, seed=3))
+    P.run_against_oracle(GossipSim, scenarios.byzantine_injectors(30_000, 16, 4, 0.2, seed=3))
 
 
 def test_single_slot_no_probing():
-    run_both(scenarios.byzantine_injectors(40_000, 12, 3, 0.05, seed=2, churn=False, slots=1))
+    P.run_against_oracle(GossipSim, scenarios.byzantine_injectors(40_000, 12, 3, 0.05, seed=2, churn=False, slots=1))
 
 
 def test_delta_variants():
-    run_both(scenarios.byzantine_injectors(20_000, 12, 3, 0.05, delta=0, seed=2, churn=False, slots=1))
-    run_both(scenarios.byzantine_injectors(20_000, 12, 3, 0.05, delta=5, seed=2))
+    P.run_against_oracle(GossipSim, scenarios.byzantine_injectors(20_000, 12, 3, 0.05, delta=0, seed=2, churn=False, slots=1))
+    P.run_against_oracle(GossipSim, scenarios.byzantine_injectors(20_000, 12, 3, 0.05, delta=5, seed=2))
 
 
 def test_injectors_and_user_events_together():
@@ -64,12 +37,10 @@ def test_injectors_and_user_events_together():
     ue = scenarios.user_event_storm(20_000, 16, 4, seed=6, n_events=3)
     sc.user_events = ue.user_events
     sc.ops += [op for op in ue.ops if (op[0], op[2]) not in {(o[0], o[2]) for o in sc.ops}]
-    g, o = run_both(sc)
-    assert g.user_event_stats() == o.user_event_stats()
-    assert (g.user_event_records() == o.user_event_records()).all()
+    P.run_against_oracle(GossipSim, sc)
 
 
 @pytest.mark.parametrize("pp", [6, 15])
 def test_injectors_with_push_pull_rounds(pp):
     """Verdicts of a tick are taken before that tick's push-pull round, on the device as in the oracle."""
-    run_both(scenarios.byzantine_injectors(30_000, 12, 3, 0.05, seed=5), push_pull_interval_ticks=pp)
+    P.run_against_oracle(GossipSim, scenarios.byzantine_injectors(30_000, 12, 3, 0.05, seed=5), push_pull_interval_ticks=pp)

@@ -10,12 +10,12 @@ import pytest
 
 import config_lib as CL
 import envelope_lib as E
+import parity_lib as P
 from oracle_lib import oracle_sim, oracle_sim_threaded
 from serf_b200 import GossipSim, MlState, scenarios
 from serf_b200.scenarios import Op, Scenario
 from serf_b200.sim import random_regular_graph
 from test_config_envelope import assert_overflow_at, overflow_scenario
-from test_emu_parity import assert_same
 
 pytestmark = pytest.mark.gpu
 
@@ -39,12 +39,9 @@ def check(jobs):
         sc = job["sc"]
         if id(sc) not in oracles:
             o = sc.build(oracle_sim_threaded if sc.n >= 100_000 else oracle_sim, trace=1, **job.get("cfg", {}))
-            oracles[id(sc)] = (o, o.run_until_converged(sc.max_ticks))
+            oracles[id(sc)] = P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
             assert CL.max_ltime(o, sc.slots) < CL.LTIME_LIMIT, sc.name
-        o, to = oracles[id(sc)]
-        what = f"{sc.name} trace={job['trace']}"
-        assert got["run"] == to, (what, got["run"], to)
-        E.assert_matches(got, o, sc.slots, with_hash=bool(job["trace"]), what=what)
+        P.assert_same(got["out"], oracles[id(sc)], with_hash=bool(job["trace"]), what=f"{sc.name} trace={job['trace']}")
     return res
 
 
@@ -96,11 +93,11 @@ def test_lifeguard_k7_full_confirmer_sets():
             assert (r == o.records(0)).all(), (trace, t)
         assert full > 100, full                                    # 8-bit confirmer masks occurred
         assert ((g.records(0)["ml"] & 3) == MlState.DEAD).sum() > n // 2
-        assert_same(g, o, 1, with_hash=bool(trace))
+        P.assert_same(P.outputs(g, sc, None), P.outputs(o, sc, None), with_hash=bool(trace))
 
 
-def _budget_check(got, limit, n):
-    m = got["stats"]["messages"]
+def _budget_check(stats, limit, n):
+    m = stats["messages"]
     assert m % limit == 0 and m // limit >= n - 1, (m, limit)           # every accepted entry sent exactly `limit` times
 
 
@@ -115,7 +112,7 @@ def test_transmit_budget_252(mult, n):
     for sc in (leave, crash):
         sc.cfg["retransmit_mult"] = mult
     res = check([dict(sc=sc, trace=t) for sc in (leave, crash) for t in (1, 0)])
-    _budget_check(res[0], limit, n)
+    _budget_check(res[0]["out"]["stats"], limit, n)
 
 
 def test_transmit_budget_248_at_the_bench_shape():
@@ -128,14 +125,9 @@ def test_transmit_budget_248_at_the_bench_shape():
     g = sc.build(device_sim, trace=0)
     tg = g.run_until_converged(sc.max_ticks)
     o = sc.build(oracle_sim_threaded, trace=0)
-    assert o.run_until_converged(sc.max_ticks) == tg
-    assert g.stats() == o.stats() and g.state_hash() == o.state_hash()
-    tr, to = g.tick_trace(), o.tick_trace()
-    for f in tr.dtype.names:
-        if f != "hash":
-            assert (tr[f] == to[f]).all(), f
-    assert (g.records(0) == o.records(0)).all() and (g.lamport_time() == o.lamport_time()).all()
-    _budget_check(dict(stats=g.stats()), limit, n - 16)
+    got = P.outputs(g, sc, tg)
+    P.assert_same(got, P.outputs(o, sc, o.run_until_converged(sc.max_ticks)), with_hash=False)
+    _budget_check(got["stats"], limit, n - 16)
 
 
 @pytest.mark.parametrize("slots", [1, 3])

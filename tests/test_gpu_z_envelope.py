@@ -14,10 +14,10 @@ SERFSIM_GRIDMUL, SERFSIM_MINB and SERFSIM_TMA_SYNC are read once per process, so
 its own (envelope_lib.run_isolated), which also reports the kernel and grid SERFSIM_VERBOSE printed for it."""
 import functools
 
-import numpy as np
 import pytest
 
 import envelope_lib as E
+import parity_lib as P
 from oracle_lib import oracle_sim, oracle_sim_threaded
 from serf_b200.sim import random_regular_graph
 from test_gpu_z_multislot_paths import MODES
@@ -37,24 +37,22 @@ _ORACLES = {}
 
 
 def oracle(sc, cfg=None):
-    """The oracle's run of a scenario (trace = 1), kept for the other variants of the same test."""
+    """The outputs of the oracle's run of a scenario (trace = 1), kept for the other variants of the same test."""
     cfg = cfg or {}
     key = (id(sc), tuple(sorted(cfg.items())))
     if key not in _ORACLES:
         o = sc.build(oracle_sim_threaded if sc.n >= 100_000 else oracle_sim, trace=1, **cfg)
-        _ORACLES[key] = (sc, o, o.run_until_converged(sc.max_ticks))          # (sc is kept alive: its id is the key)
-    return _ORACLES[key][1:]
+        _ORACLES[key] = (sc, P.outputs(o, sc, o.run_until_converged(sc.max_ticks)))          # (sc is kept alive: its id is the key)
+    return _ORACLES[key][1]
 
 
 def check(jobs, env, expect_kernel=None):
     """Run the jobs in a fresh process under env and compare each with the oracle; returns the outputs."""
     res = E.run_isolated(jobs, env)
     for job, got in zip(jobs, res):
-        sc, cfg = job["sc"], job.get("cfg", {})
-        o, to = oracle(sc, cfg)
+        sc = job["sc"]
         what = f"{sc.name} trace={job['trace']} {env}"
-        assert got["run"] == to, (what, got["run"], to)
-        E.assert_matches(got, o, sc.slots, with_hash=bool(job["trace"]), what=what)
+        P.assert_same(got["out"], oracle(sc, job.get("cfg", {})), with_hash=bool(job["trace"]), what=what)
         if expect_kernel:
             assert E.is_kernel(got["kernel"][0], expect_kernel), (what, got["kernel"])
     return res
@@ -89,7 +87,7 @@ def test_uniform_graph_forced_through_general_path():
     a = check(both(sc), {})
     b = check(both(sc), {"SERFSIM_UDEG": "0"})
     for x, y in zip(a, b):
-        assert (x["trace"] == y["trace"]).all() and x["hash"] == y["hash"]
+        P.assert_same(y["out"], x["out"], with_hash=True, what="SERFSIM_UDEG=0")
 
 
 # ---- TMA stage boundary ---------------------------------------------------------------------------------------------
@@ -155,10 +153,7 @@ def test_scheduler_switches(env):
     studies, fz = switch_scenarios()
     res = check(both(*studies) + [dict(sc=sc, trace=0) for sc in fz], env)
     for got, base in zip(res, default_switch_runs()):
-        assert (got["trace"] == base["trace"]).all() and got["hash"] == base["hash"] and got["run"] == base["run"]
-        for s in range(16):
-            if f"rec{s}" in got:
-                assert (got[f"rec{s}"] == base[f"rec{s}"]).all()
+        P.assert_same(got["out"], base["out"], with_hash=True, what=str(env))
 
 
 # ---- fan-out 6–8 × slots 9–16 -------------------------------------------------------------------------------------------

@@ -4,24 +4,12 @@ raised if a view outside a one-element set of views with business turns out to h
 mode, a crash + leave study with LAN-like timers, multi-phase sequences (converge → crash → continue → rejoin), fuzz scenarios."""
 import pytest
 
+import parity_lib as P
 from oracle_lib import oracle_sim
 from serf_b200 import GossipSim, scenarios
 from serf_b200.sim import Op
 
 pytestmark = pytest.mark.gpu
-
-
-def same(g, o, slots, with_hash):
-    assert g.stats() == o.stats()
-    n = o.stats()["tick"]
-    tg, to = g.tick_trace(0, n), o.tick_trace(0, n)
-    for f in tg.dtype.names:
-        if f != "hash" or with_hash:
-            assert (tg[f] == to[f]).all(), f
-    assert g.state_hash() == o.state_hash()
-    for s in range(slots):
-        assert (g.records(s) == o.records(s)).all()
-    assert (g.lamport_time() == o.lamport_time()).all()
 
 
 MODES = [dict(SERFSIM_SV="0", SERFSIM_AHEAD="0"), dict(SERFSIM_SV="1", SERFSIM_AHEAD="2"), dict(SERFSIM_SV="2", SERFSIM_AHEAD="1"),
@@ -33,12 +21,7 @@ def test_crash_and_leave_study(monkeypatch, mode):
     for k, v in mode.items():
         monkeypatch.setenv(k, v)
     for sc in (scenarios.dissemination_storm(200_000, 16, 4, slots=2, seed=3, with_fail=True), scenarios.dissemination_storm(60_000, 12, 3, slots=3, seed=5, with_fail=True)):
-        o = sc.build(oracle_sim, trace=1)
-        to = o.run_until_converged(sc.max_ticks)
-        for trace in (0, 1):
-            g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), trace=trace)
-            assert g.run_until_converged(sc.max_ticks) == to
-            same(g, o, sc.slots, with_hash=bool(trace))
+        P.run_against_oracle(GossipSim, sc, traces=(0, 1))
 
 
 @pytest.mark.parametrize("mode", MODES[1:3], ids=lambda m: ",".join(f"{k[8:]}={v}" for k, v in m.items()))
@@ -49,22 +32,22 @@ def test_multi_phase(monkeypatch, mode, seed):
     monkeypatch.setenv("SERFSIM_CHUNK", "5")
     sc = scenarios.random_graph_leave(40_000, 12, 4, seed=seed, slots=3, graph_seed=seed + 30)
     cfg = dict(suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
-    g, o = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), trace=0, **cfg), sc.build(oracle_sim, trace=1, **cfg)
+    g, o = sc.build(GossipSim, trace=0, **cfg), sc.build(oracle_sim, trace=1, **cfg)
     assert g.run_until_converged(sc.max_ticks) == o.run_until_converged(sc.max_ticks)
     for sim in (g, o):
         sim.inject(sim.stats()["tick"], Op.FAIL, int(sc.subjects[1]), 0)           # from here on exactly one subject has ever been down
-    assert g.run_until_converged(5000) == o.run_until_converged(5000)
-    same(g, o, sc.slots, with_hash=False)
+    tg, to = g.run_until_converged(5000), o.run_until_converged(5000)
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=False)
     for sim in (g, o):
         t = sim.stats()["tick"]
         sim.inject(t, Op.REJOIN, int(sc.subjects[1]), 0)
         sim.inject(t + 2, Op.FORCE_LEAVE, 11, 2)
-    assert g.run_until_converged(5000) == o.run_until_converged(5000)
-    same(g, o, sc.slots, with_hash=False)
+    tg, to = g.run_until_converged(5000), o.run_until_converged(5000)
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=False)
     for sim in (g, o):
         sim.inject(sim.stats()["tick"] + 1, Op.FAIL, int(sc.subjects[2]), 0)       # a second subject goes down: the dispatch switches itself off
-    assert g.run_until_converged(5000) == o.run_until_converged(5000)
-    same(g, o, sc.slots, with_hash=False)
+    tg, to = g.run_until_converged(5000), o.run_until_converged(5000)
+    P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=False)
 
 
 @pytest.mark.parametrize("mode", MODES[1:3], ids=lambda m: ",".join(f"{k[8:]}={v}" for k, v in m.items()))
@@ -72,9 +55,4 @@ def test_fuzz(monkeypatch, mode):
     for k, v in mode.items():
         monkeypatch.setenv(k, v)
     for seed in range(8):
-        sc = scenarios.fuzz(seed)
-        o = sc.build(oracle_sim, trace=1)
-        to = o.run_until_converged(sc.max_ticks)
-        g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), trace=0)
-        assert g.run_until_converged(sc.max_ticks) == to
-        same(g, o, sc.slots, with_hash=False)
+        P.run_against_oracle(GossipSim, scenarios.fuzz(seed), traces=(0,))

@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 import envelope_lib as E
+import parity_lib as P
 import scaled_fuzz_lib as S
 from oracle_lib import oracle_sim, oracle_sim_threaded
 from serf_b200 import GossipSim
@@ -39,12 +40,12 @@ def oracle(seed):
     """One oracle run (trace = 1) per seed, shared by every mode."""
     sc = scenario(seed)
     o = sc.build(oracle_sim_threaded if sc.n >= 100_000 else oracle_sim, trace=1)
-    return sc, S.oracle_outputs(o, sc, o.run_until_converged(sc.max_ticks))
+    return sc, P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
 
 
 def run(sc, trace):
-    g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), trace=trace)
-    out = S.outputs(g, sc, g.run_until_converged(sc.max_ticks))
+    g = sc.build(GossipSim, trace=trace)
+    out = E.product_run(g, sc)
     g.close()
     return out
 
@@ -53,7 +54,7 @@ def run(sc, trace):
 def production(seed):
     sc, ref = oracle(seed)
     got = run(sc, 0)
-    S.assert_same_outputs(got, ref, sc, with_hash=False, what=f"{sc.name} trace=0")
+    P.assert_same(got["out"], ref, with_hash=False, what=f"{sc.name} trace=0")
     return got
 
 
@@ -61,7 +62,7 @@ def production(seed):
 def test_scaled_fuzz(seed):
     sc, ref = oracle(seed)
     assert sc.n % E.TILE != 0
-    S.assert_same_outputs(run(sc, 1), ref, sc, with_hash=True, what=f"{sc.name} trace=1")
+    P.assert_same(run(sc, 1)["out"], ref, with_hash=True, what=f"{sc.name} trace=1")
     production(seed)
 
 
@@ -85,7 +86,7 @@ def test_jumps_launch_fewer_kernels(monkeypatch):
         monkeypatch.setenv("SERFSIM_NO_JUMP", "1")
         nj = run(sc, 0)
         monkeypatch.delenv("SERFSIM_NO_JUMP")
-        S.assert_same_outputs(nj, ref, sc, with_hash=False, what=f"{sc.name} NO_JUMP")
+        P.assert_same(nj["out"], ref, with_hash=False, what=f"{sc.name} NO_JUMP")
         assert base["launches"] <= nj["launches"], (sc.name, base["launches"], nj["launches"])
         jumped += base["launches"] < nj["launches"]
     assert jumped >= 2, jumped
@@ -103,7 +104,7 @@ def test_mode_matrix(mode, monkeypatch):
         for k, v in mode.items():
             monkeypatch.setenv(k, str(3 + i % 5) if v == "chunk" else v)
         got = run(sc, 0)
-        S.assert_same_outputs(got, ref, sc, with_hash=False, what=f"{sc.name} {mode}")
+        P.assert_same(got["out"], ref, with_hash=False, what=f"{sc.name} {mode}")
         if mode.get("SERFSIM_SV") in ("0", "2"):
             assert not got["view_kinds"].any()                     # no tick ran as passes
 
@@ -115,7 +116,7 @@ def test_tma_on_single_slot_seeds(monkeypatch):
     for seed in scs:
         sc, ref = oracle(seed)
         for trace in (1, 0):
-            S.assert_same_outputs(run(sc, trace), ref, sc, with_hash=bool(trace), what=f"{sc.name} TMA trace={trace}")
+            P.assert_same(run(sc, trace)["out"], ref, with_hash=bool(trace), what=f"{sc.name} TMA trace={trace}")
 
 
 def test_several_tiles_per_cta():
@@ -126,5 +127,5 @@ def test_several_tiles_per_cta():
     res = E.run_isolated([dict(sc=oracle(s)[0], trace=t) for s in seeds for t in (1, 0)], {"SERFSIM_GRIDMUL": "1"})
     for i, got in enumerate(res):
         sc, ref = oracle(seeds[i // 2])
-        S.assert_same_outputs(got, ref, sc, with_hash=i % 2 == 0, what=f"{sc.name} GRIDMUL=1")
+        P.assert_same(got["out"], ref, with_hash=i % 2 == 0, what=f"{sc.name} GRIDMUL=1")
         assert E.tiles_per_cta(sc.n, got["kernel"][1]) > 1, (sc.name, got["kernel"])

@@ -2,79 +2,45 @@
 literal ring-buffer model, bit for bit — 16-byte event records, event clocks, stamped Lamport times, every trace row
 (user-event deliveries are part of edge_updates / messages / changed / pending / hash), counters and the state hash.
 """
-import numpy as np
 import pytest
 
-from oracle_lib import oracle_sim
-from serf_b200 import scenarios
-from test_gpu_parity import assert_same, gpu_sim
+import parity_lib as P
+from serf_b200 import GossipSim, scenarios
 
 pytestmark = pytest.mark.gpu
 
 
-def assert_same_events(g, o, n_events):
-    rg, ro = g.user_event_records(), o.user_event_records()
-    bad = np.nonzero(rg != ro)[0]
-    assert bad.size == 0, f"event record of node {bad[0]} differs: gpu {rg[bad[0]]} oracle {ro[bad[0]]}"
-    assert g.user_event_stats() == o.user_event_stats(), (g.user_event_stats(), o.user_event_stats())
-    assert (g.event_time() == o.event_time()).all()
-    for e in range(n_events):
-        assert g.user_event_ltime(e) == o.user_event_ltime(e)
-        assert (g.user_event_seen(e) == o.user_event_seen(e)).all()
-
-
-def run_both(sc, **cfg):
-    E = len(sc.user_events)
-    o = sc.build(oracle_sim, trace=1, **cfg)
-    to = o.run_until_converged(sc.max_ticks)
-    g = sc.build(gpu_sim, trace=1, **cfg)
-    assert g.run_until_converged(sc.max_ticks) == to
-    assert_same(g, o, sc.slots)
-    assert_same_events(g, o, E)
-    f = sc.build(gpu_sim, trace=0, **cfg)                 # production mode: idle nodes stop after 20 bytes, no per-tick hash
-    assert f.run_until_converged(sc.max_ticks) == to
-    n = o.stats()["tick"]
-    trf, tro = f.tick_trace(0, n), o.tick_trace(0, n)
-    for name in trf.dtype.names:
-        if name != "hash":
-            bad = np.nonzero(trf[name] != tro[name])[0]
-            assert bad.size == 0, f"trace=0: field {name} first differs at tick {bad[0]}"
-    assert f.state_hash() == o.state_hash() and f.stats() == o.stats()
-    assert_same_events(f, o, E)
-    return g, o
-
-
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_user_event_storm_100k(seed):
-    g, o = run_both(scenarios.user_event_storm(100_000, 16, 3, seed=seed, n_events=4, spacing=3))
-    assert g.user_event_stats()["event_queue"] == 0
+    out = P.run_against_oracle(GossipSim, scenarios.user_event_storm(100_000, 16, 3, seed=seed, n_events=4, spacing=3))
+    assert out["user_event_stats"]["event_queue"] == 0
 
 
 def test_user_events_with_churn_and_leave():
-    run_both(scenarios.user_event_storm(40_000, 16, 3, seed=4, n_events=6, spacing=1, churn=300, with_leave=True))
+    P.run_against_oracle(GossipSim, scenarios.user_event_storm(40_000, 16, 3, seed=4, n_events=6, spacing=1, churn=300, with_leave=True))
 
 
 def test_aliased_events():
-    g, o = run_both(scenarios.user_event_storm(30_000, 12, 3, seed=5, n_events=3, spacing=2, alias=True))
-    both = g.user_event_seen(0) + g.user_event_seen(1)
+    out = P.run_against_oracle(GossipSim, scenarios.user_event_storm(30_000, 12, 3, seed=5, n_events=3, spacing=2, alias=True))
+    both = out["user_event_seen"][0] + out["user_event_seen"][1]
     assert (both <= 1).all() and (both == 1).mean() > 0.999           # never both; a random digraph may strand a node or two with neither
 
 
 @pytest.mark.parametrize("fanout,events", [(1, 2), (4, 8), (8, 3)])
 def test_fanouts_and_event_counts(fanout, events):
-    run_both(scenarios.user_event_storm(20_000, 10, fanout, seed=7, n_events=events, spacing=1, churn=50))
+    P.run_against_oracle(GossipSim, scenarios.user_event_storm(20_000, 10, fanout, seed=7, n_events=events, spacing=1, churn=50))
 
 
 def test_user_events_with_failure_detection():
     """Probing on, a tracked subject down: the membership kernel runs its watcher path while events are in flight."""
     sc = scenarios.user_event_storm(20_000, 16, 3, seed=8, n_events=4, spacing=4, with_leave=False)
     sc.ops.append((2, scenarios.Op.FAIL, 0, 0))
-    run_both(sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
+    P.run_against_oracle(GossipSim, sc, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
 
 
 def test_reset_clears_event_state():
     sc = scenarios.user_event_storm(5_000, 12, 3, seed=2, n_events=3)
-    g = sc.build(gpu_sim, trace=1)
+    g = sc.build(GossipSim, trace=1)
     g.run_until_converged(sc.max_ticks)
     h1, st1 = g.state_hash(), g.user_event_stats()
     g.reset(sc.cfg["seed"])
@@ -87,7 +53,7 @@ def test_reset_clears_event_state():
 @pytest.mark.parametrize("pp", [5, 13])
 def test_user_events_with_push_pull_rounds(pp):
     """retransmit_mult 1 leaves the gossip of the events incomplete; push-pull rounds replay the partner's event ring."""
-    run_both(scenarios.user_event_storm(30_000, 8, 2, seed=6, n_events=5, spacing=2, churn=100, with_leave=True), push_pull_interval_ticks=pp, retransmit_mult=1)
+    P.run_against_oracle(GossipSim, scenarios.user_event_storm(30_000, 8, 2, seed=6, n_events=5, spacing=2, churn=100, with_leave=True), push_pull_interval_ticks=pp, retransmit_mult=1)
 
 
 @pytest.mark.parametrize("seed", range(12))
@@ -95,18 +61,4 @@ def test_fuzz_with_user_events_and_injectors(seed):
     """Every operation kind, reaper, probing, tracked user events (with aliases) and byzantine injectors at once."""
     sc = scenarios.fuzz_features(seed)
     sc.max_ticks = 1200
-    o = sc.build(oracle_sim, trace=1)
-    to = o.run_until_converged(sc.max_ticks)
-    for trace in (1, 0):
-        g = sc.build(gpu_sim, trace=trace)
-        assert g.run_until_converged(sc.max_ticks) == to
-        if trace:
-            assert_same(g, o, sc.slots)
-        else:
-            assert g.state_hash() == o.state_hash() and g.stats() == o.stats()
-        if sc.user_events is not None:
-            assert g.user_event_stats() == o.user_event_stats()
-            assert (g.user_event_records() == o.user_event_records()).all()
-        if sc.byzantine is not None:
-            assert g.byzantine_stats() == o.byzantine_stats()
-            assert (g.anomaly_flags() == o.anomaly_flags()).all()
+    P.run_against_oracle(GossipSim, sc)

@@ -262,7 +262,7 @@ def test_content_table_rules():
 
 
 def test_sharded_batches_concatenate_to_the_single_batch():
-    from test_emu_multi import ThreadComm
+    from parity_lib import ThreadComm
     sc = scenarios.user_event_storm(1800, 8, 3, seed=3, n_events=4, spacing=2, churn=20)
     ticks = 25
     g1 = sc.build(emu_sim, trace=0)

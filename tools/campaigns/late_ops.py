@@ -2,15 +2,11 @@
 host operations — many of them no-ops — scattered over the 300 ticks AFTER the busy part, where the cluster sleeps between timers, reaper and
 anti-entropy rounds.  Host-compiled kernels (tests/emu) against the oracle, production mode and trace mode, default launch chunks and a random
 fixed chunk; single rank and two ranks.  Prints the failing seeds (none expected)."""
-import sys, time, os, threading
+import sys, time, os
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
-import numpy as np
+import parity_lib as P
 from emu_lib import emu_sim
 from oracle_lib import oracle_sim
-from serf_b200 import scenarios
-from serf_b200.sim import Op
-import test_emu_parity as P
-import test_emu_multi as M
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 from late_ops_gen import late
@@ -19,24 +15,15 @@ bad = []; t_start = time.time()
 for seed in range(1000, 1400):
     sc = late(seed)
     try:
-        o = sc.build(oracle_sim, trace=1); to = o.run_until_converged(sc.max_ticks)
+        o = sc.build(oracle_sim, trace=1); ref = P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
         for trace, chunk in ((0, None), (1, None), (0, str(2 + seed % 11))):
             if chunk: os.environ["SERFSIM_CHUNK"] = chunk
             else: os.environ.pop("SERFSIM_CHUNK", None)
             g = sc.build(emu_sim, trace=trace)
-            tg = g.run_until_converged(sc.max_ticks)
-            assert tg == to, (tg, to, trace, chunk)
-            P.assert_same(g, o, sc.slots, with_hash=bool(trace))
+            P.assert_same(P.outputs(g, sc, g.run_until_converged(sc.max_ticks)), ref, with_hash=bool(trace), what=f"trace={trace} chunk={chunk}")
         os.environ.pop("SERFSIM_CHUNK", None)
         if seed % 3 == 0:                                   # two ranks, production mode
-            res = M.run_sharded(sc, 2, trace=0)
-            tro = o.tick_trace(0, o.stats()["tick"])
-            for r in res:
-                assert (r["ticks"], r["ok"]) == to, (r["ticks"], r["ok"], to)
-                for f in tro.dtype.names:
-                    if f != "hash": assert (r["trace"][f] == tro[f]).all(), f
-            for s in range(sc.slots):
-                assert (np.concatenate([r["rec"][s] for r in res]) == o.records(s)).all()
+            P.assert_same(P.run_ranks(sc, 2, 0), ref, with_hash=False, what="2 ranks")
     except Exception as e:
         bad.append((seed, repr(e)[:160])); print("FAIL", seed, repr(e)[:160], flush=True)
     if time.time() - t_start > 1500: break

@@ -1,11 +1,9 @@
 """Randomized campaign of fuzz / fuzz_features scenarios beyond the committed seeds: host-compiled kernels (tests/emu) vs oracle.
 Run from the repo root; prints the failing seeds (none expected).  Takes 10-20 minutes."""
-import sys, time, threading
+import sys, time
 import os; ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
-import numpy as np
-import test_emu_multi as M
+import parity_lib as P
 from emu_lib import emu_sim
-from oracle_lib import oracle_sim
 from serf_b200 import scenarios
 bad=[]; t0=time.time(); n_done=0
 for seed in range(100, 400):
@@ -13,35 +11,7 @@ for seed in range(100, 400):
     sc.max_ticks = 300
     world = 2 + seed % 3
     try:
-        o = sc.build(oracle_sim, trace=1); to, oko = o.run_until_converged(sc.max_ticks)
-        tro = o.tick_trace()
-        for trace in (0,):
-            comm = M.ThreadComm(world); res=[None]*world; errs=[]
-            def worker(rank):
-                try:
-                    g = sc.build(emu_sim, rank=rank, world_size=world, trace=trace)
-                    g.connect(*comm.hooks(rank))
-                    t = g.run_until_converged(sc.max_ticks)
-                    r = dict(t=t, trace=g.tick_trace(), hash=g.state_hash(), rec=[g.records(s) for s in range(sc.slots)])
-                    if sc.user_events is not None: r['ue']=g.user_event_records(); r['ues']=g.user_event_stats()
-                    if sc.byzantine is not None: r['fl']=g.anomaly_flags(); r['bs']=g.byzantine_stats()
-                    res[rank]=r; comm.bar.wait()
-                except BaseException as e:
-                    errs.append(e); comm.bar.abort()
-            th=[threading.Thread(target=worker,args=(r,)) for r in range(world)]
-            [t.start() for t in th]; [t.join(600) for t in th]
-            if errs: raise errs[0]
-            for r in res:
-                assert r['t']==(to,oko), (r['t'],(to,oko))
-                for f in tro.dtype.names:
-                    if f!='hash': assert (r['trace'][f]==tro[f]).all(), f
-                assert r['hash']==o.state_hash()
-            for s in range(sc.slots): assert (np.concatenate([r['rec'][s] for r in res])==o.records(s)).all()
-            if sc.user_events is not None:
-                assert (np.concatenate([r['ue'] for r in res])==o.user_event_records()).all()
-            if sc.byzantine is not None:
-                assert (np.concatenate([r['fl'] for r in res])==o.anomaly_flags()).all()
-                assert all(r['bs']==o.byzantine_stats() for r in res)
+        P.run_against_oracle(emu_sim, sc, traces=(0,), world=world)
         n_done+=1
     except Exception as e:
         bad.append((seed, repr(e)[:200])); print('FAIL', seed, world, repr(e)[:300], flush=True)

@@ -3,21 +3,14 @@ Run from the repo root; prints the failing seeds (none expected).  Takes 10-20 m
 import sys, time
 import os; ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 from emu_lib import emu_sim
-from oracle_lib import oracle_sim
 from serf_b200 import scenarios
-import test_emu_parity as P
-import numpy as np
+import parity_lib as P
 bad=[]
 t0=time.time()
 def one(sc, tag):
     sc.max_ticks=min(sc.max_ticks,1500)
     try:
-        o = sc.build(oracle_sim, trace=1); to=o.run_until_converged(sc.max_ticks)
-        for trace in (0,1):
-            g = sc.build(emu_sim, trace=trace)
-            assert g.run_until_converged(sc.max_ticks)==to
-            P.assert_same(g,o,sc.slots,with_hash=bool(trace))
-            P._feature_checks(g,o,sc)
+        P.run_against_oracle(emu_sim, sc, traces=(0, 1))
     except Exception as e:
         bad.append((tag, repr(e)[:200])); print('FAIL', tag, repr(e)[:200], flush=True)
 for s in range(40, 400):

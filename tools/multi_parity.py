@@ -2,9 +2,9 @@
 """Sharded parity on real GPUs in ONE process group per world size (launch under torchrun): every scenario of
 tests/test_gpu_multi.py — membership, failure detection, fuzz, user events, injectors, push-pull rounds across shards — plus,
 with --full, BASELINE configs[4] at its stated size (10 M nodes, 100 000 injectors).  Rank 0 runs the (threaded) oracle and
-compares: convergence tick, every row of the (global) trace, state hash, records of every slot, clocks, event records and
-counters, anomaly flags.  One line per scenario; exit code 1 if anything differs.  The same comparisons as the pytest file, without
-paying the NCCL start-up once per case (GPU minutes on a multi-GPU box are charged per GPU).
+compares every output of tests/parity_lib.py (the raw records only below 500 K nodes: the state hash covers them above).  One line
+per scenario; exit code 1 if anything differs.  The same comparisons as the pytest file, without paying the NCCL start-up once per
+case (GPU minutes on a multi-GPU box are charged per GPU).
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 tools/multi_parity.py [--full]
 """
@@ -12,7 +12,6 @@ import os
 import sys
 import time
 
-import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -21,6 +20,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from serf_b200 import GossipSim, scenarios  # noqa: E402
 from serf_b200 import dist as sdist  # noqa: E402
+import parity_lib as P  # noqa: E402
 
 rank, world, lr = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
 torch.cuda.set_device(lr)
@@ -51,48 +51,21 @@ for name, kwargs, cfg in CASES:
     sc = getattr(scenarios, name)(**kwargs)
     big = sc.n > 500_000
     trace = 0 if big else 1
-    g = sc.build(lambda n, s, **kw: GossipSim(n, s, **kw), device=lr, rank=rank, world_size=world, trace=trace, **cfg)
+    g = sc.build(GossipSim, device=lr, rank=rank, world_size=world, trace=trace, **cfg)
     sdist.connect(g, dist, torch.device("cuda", lr))
-    ticks, ok = g.run_until_converged(sc.max_ticks)
-    # collective getters: every rank makes the same calls in the same order
-    tr, h, clock = g.tick_trace(), g.state_hash(), (g.lamport_time_u32() if big else g.lamport_time())
-    recs = [g.records(s) for s in range(sc.slots)] if not big else []
-    status = [g.member_status(s) for s in range(sc.slots)]
-    ue = (g.user_event_records(), g.user_event_stats(), [g.user_event_ltime(e) for e in range(len(sc.user_events))]) if sc.user_events is not None else None
-    bz = (g.anomaly_flags(), g.byzantine_stats()) if sc.byzantine is not None else None
+    out = P.outputs(g, sc, g.run_until_converged(sc.max_ticks), records=not big)
     parts = [None] * world
-    dist.gather_object(dict(clock=clock, recs=recs, status=status, ue=ue[0] if ue else None, flags=bz[0] if bz else None, ticks=(ticks, ok), trace=tr, hash=h,
-                            ue_stats=ue[1] if ue else None, ue_lt=ue[2] if ue else None, bz_stats=bz[1] if bz else None), parts if rank == 0 else None, dst=0)
+    dist.gather_object(out, parts if rank == 0 else None, dst=0)
     msg = "ok"
     if rank == 0:
         from oracle_lib import oracle_sim, oracle_sim_threaded
         o = sc.build(oracle_sim_threaded if big else oracle_sim, trace=trace, **cfg)
         to = o.run_until_converged(sc.max_ticks)
-        n = o.stats()["tick"]
-        tro = o.tick_trace(0, n)
-        errs = []
-        for r, p in enumerate(parts):
-            if tuple(p["ticks"]) != tuple(to): errs.append(f"rank {r}: converged {p['ticks']} vs {to}")
-            for f in tro.dtype.names:
-                if f == "hash" and not trace: continue
-                if len(p["trace"]) != len(tro) or (p["trace"][f] != tro[f]).any(): errs.append(f"rank {r}: trace field {f}"); break
-            if int(p["hash"]) != o.state_hash(): errs.append(f"rank {r}: state hash")
-        if (np.concatenate([p["clock"] for p in parts]) != o.lamport_time()).any(): errs.append("clocks")
-        for s in range(sc.slots):
-            if not big and (np.concatenate([p["recs"][s] for p in parts]) != o.records(s)).any(): errs.append(f"records slot {s}")
-            if (np.concatenate([p["status"][s] for p in parts]) != o.member_status(s)).any(): errs.append(f"status slot {s}")
-        if sc.user_events is not None:
-            if (np.concatenate([p["ue"] for p in parts]) != o.user_event_records()).any(): errs.append("event records")
-            so = o.user_event_stats()
-            for p in parts:
-                if {k: v for k, v in p["ue_stats"].items() if k != "event_time"} != {k: v for k, v in so.items() if k != "event_time"}: errs.append("event stats"); break
-                if [int(x) for x in p["ue_lt"]] != [o.user_event_ltime(e) for e in range(len(sc.user_events))]: errs.append("event ltimes"); break
-        if sc.byzantine is not None:
-            if (np.concatenate([p["flags"] for p in parts]) != o.anomaly_flags()).any(): errs.append("anomaly flags")
-            if any(p["bz_stats"] != o.byzantine_stats() for p in parts): errs.append("byzantine stats")
-        if errs:
+        try:
+            P.assert_same(P.merge_ranks(parts), P.outputs(o, sc, to, records=not big), with_hash=bool(trace))
+        except AssertionError as e:
             failed += 1
-            msg = "FAILED: " + "; ".join(errs[:4])
+            msg = f"FAILED: {e}"[:400]
         print(f"world {world}  {sc.name:38s} {cfg if cfg else ''}  ticks {to}  {time.time() - t0:5.1f} s  {msg}", flush=True)
     g.close()
     dist.barrier()
