@@ -102,6 +102,56 @@ std::vector<u32> suspicion_table(u32 susp_mult, u32 max_mult, u32 probe_ticks, u
   return tab;
 }
 
+// Run-time switches: every SERFSIM_* environment variable the library reads, read once per handle by read_switches (serfsim_create).
+// Defaults are the measured-fastest settings; the switches exist for A/B measurements and debugging and never change results.
+struct Switches {
+  int gridmul = 2;            // SERFSIM_GRIDMUL >= 1 (else 2): waves of resident CTAs in the tick kernels' persistent grid
+  bool minb5 = false;         // SERFSIM_MINB=5: single-slot runs size their grid for 5 CTAs/SM, and unsharded ones launch the 5-CTA instance
+  bool tma = false;           // SERFSIM_TMA=1: single-slot runs stage tiles through the TMA pipeline if a tile's CSR span fits 48 KB
+  bool tma_sync = false;      // SERFSIM_TMA_SYNC=1: the TMA pipeline's barrier-synchronised form
+  bool udeg = true;           // SERFSIM_UDEG=0: row offsets are loaded even when every row has the same degree (the general path)
+  u32 ahead = 1;              // SERFSIM_AHEAD=0|1|2: multi-slot kernel requests one tile ahead off / in saturated ticks / always
+  u32 sv = 1;                 // SERFSIM_SV=0|1|2: multi-slot ticks as per-view passes (sharded: single-view dual launch) off / on / check mode
+  bool compact = true;        // SERFSIM_COMPACT=0: tile-by-tile walk in unsaturated ticks too
+  bool dedup = true;          // SERFSIM_DEDUP=0: unsharded sends issue every RED, also those that change nothing
+  bool no_skip = false;       // SERFSIM_NO_SKIP=1: process every tile, every view, every tick
+  bool no_jump = false;       // SERFSIM_NO_JUMP (set): the convergence loop launches the ticks the cluster sleeps through
+  u32 chunk = 0;              // SERFSIM_CHUNK=n (>= 1): ticks per launch chunk; 0 (unset): 8, doubling up to 32, 8 again after a jump
+  double win_factor = 1.25;   // SERFSIM_WIN_FACTOR=x: sharded receive windows hold x times the expected entries per tick and peer
+  bool no_fuse = false;       // SERFSIM_NO_FUSE (set): sharded ticks launch a separate publish kernel instead of the fused one
+  int l2_persist = 0;         // SERFSIM_L2_PERSIST != 0: set aside the largest persisting L2 carve-out (off: it takes L2 from every plane)
+  bool l2_window = false;     // SERFSIM_L2_WINDOW=1: stream access-policy window over the inbox being written
+  bool verbose = false;       // SERFSIM_VERBOSE (set): print the L2 limits and the tick kernel and grid picked for each topology
+  bool debug_loop = false;    // SERFSIM_DEBUG_LOOP (set): print the convergence loop's state after every launch chunk
+  bool xtiming = false;       // SERFSIM_XTIMING (set): serfsim_destroy prints the tick kernel / exchange split of a timed sharded run
+};
+
+Switches read_switches() {
+  auto num = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
+  auto set = [](const char* name) { return getenv(name) != nullptr; };
+  Switches s;
+  s.gridmul = num("SERFSIM_GRIDMUL", s.gridmul); if (s.gridmul < 1) s.gridmul = 2;
+  s.minb5 = num("SERFSIM_MINB", 0) == 5;
+  s.tma = num("SERFSIM_TMA", s.tma) != 0;
+  s.tma_sync = num("SERFSIM_TMA_SYNC", s.tma_sync) != 0;
+  s.udeg = num("SERFSIM_UDEG", s.udeg) != 0;
+  s.ahead = (u32)std::min(2, std::max(0, num("SERFSIM_AHEAD", s.ahead)));
+  s.sv = (u32)std::min(2, std::max(0, num("SERFSIM_SV", s.sv)));
+  s.compact = num("SERFSIM_COMPACT", s.compact) != 0;
+  s.dedup = num("SERFSIM_DEDUP", s.dedup) != 0;
+  s.no_skip = num("SERFSIM_NO_SKIP", s.no_skip) != 0;
+  s.no_jump = set("SERFSIM_NO_JUMP");
+  s.chunk = set("SERFSIM_CHUNK") ? (u32)std::max(1, num("SERFSIM_CHUNK", 1)) : 0u;
+  if (const char* e = getenv("SERFSIM_WIN_FACTOR")) s.win_factor = atof(e);
+  s.no_fuse = set("SERFSIM_NO_FUSE");
+  s.l2_persist = num("SERFSIM_L2_PERSIST", s.l2_persist);
+  s.l2_window = num("SERFSIM_L2_WINDOW", s.l2_window) != 0;
+  s.verbose = set("SERFSIM_VERBOSE");
+  s.debug_loop = set("SERFSIM_DEBUG_LOOP");
+  s.xtiming = set("SERFSIM_XTIMING");
+  return s;
+}
+
 }  // namespace
 
 struct serfsim {
@@ -135,7 +185,6 @@ struct serfsim {
   u64* d_trace = nullptr;          // [trace_cap][8]
   u32* d_kinds = nullptr;          // [trace_cap+1][4]; row t+1 = messages by kind sent in tick t
   u32* d_view_kinds = nullptr;     // [trace_cap+1][R][4]; row t+1 = messages by view and kind sent in tick t by per-view passes (zero otherwise)
-  u32* d_ones = nullptr;           // [4] non-zero (multi-GPU: never skip an inbox plane)
   u32 trace_cap = 0;
   u32* d_overflow = nullptr;       // device address of pin_overflow (mapped pinned host memory: written by kernels on the rare error paths, read by the host without a copy)
   u32* pin_overflow = nullptr;
@@ -170,13 +219,11 @@ struct serfsim {
   std::vector<u32> subj;
   u32 up_mask = 0;
   u32 ever_down = 0;               // subjects that have been down at some tick since the reset (only those are probed, suspected, run timers)
-  u32 sv = 1;                      // multi-slot runs: 1 = per-view passes (sharded: single-view dual launch), 2 = check mode, 0 = off (SERFSIM_SV, tick_kernel.cuh)
   int grid_sv = 0;                 // grid of the single-view kernel
   u32 tick = 0;
   bool has_topo = false;
   u32 stage_col_bytes = 0;         // 0: direct-load kernel; else bytes of CSR per TMA stage
   u32 max_tile_edges = 0;          // largest 16-byte-aligned CSR span of one 256-node tile (sizes the TMA stage)
-  u32 ahead = 1;                   // multi-slot tick kernel: software pipelining of saturated ticks (SERFSIM_AHEAD=0 / 1 / 2, tick_kernel.cuh)
   u32 udeg = 0;                    // uniform out-degree of the shard's rows (0: degrees differ)
   std::vector<serfsim_tick_row_t> rows;   // rows pulled from the device so far (global sums when sharded)
   // device-side convergence gate (tick_kernel.cuh: Gate)
@@ -197,7 +244,9 @@ struct serfsim {
   void* cb_user = nullptr;
   std::vector<u8> reported;        // last status reported per slot
   int grid = 1;
-  int ctas_per_sm = 4;
+  int ctas_per_sm = 4;             // resident CTAs per SM the membership kernel's grid is sized for (and its __launch_bounds__ instance)
+  int sms = 132;                   // the device's SM count
+  Switches sw;                     // run-time switches, read at serfsim_create
   // multi-GPU
   u64* d_win_data[2] = {nullptr, nullptr};     // my receive windows [parity][world][win_cap]  (IPC-exported)
   u32* d_ctrl = nullptr;                       // my control block [parity][counts[8] | flags[8]] (IPC-exported)
@@ -213,10 +262,6 @@ struct serfsim {
   std::vector<void*> ipc_opened;
   bool tick_timing = false;
   size_t l2_persist_max = 0, l2_window_max = 0;
-  bool l2_window = false;           // SERFSIM_L2_WINDOW=1: stream access-policy window over the inbox being written
-  bool no_skip = false;             // SERFSIM_NO_SKIP=1: process every tile every tick (A/B measurements)
-  bool compact = true;              // SERFSIM_COMPACT=0: tile-by-tile walk in unsaturated ticks too (A/B measurements)
-  bool dedup = true;                // SERFSIM_DEDUP=0: unsharded sends issue every RED, also those that change nothing (A/B measurements)
   // asynchronous result read-back (serfsim_results_async): extraction into a ring of staging buffers on the launch stream,
   // device→host copies on a second stream so that they overlap the ticks of the caller's next step
   struct ResBuf { unsigned char* d = nullptr; cudaEvent_t copied = nullptr; bool used = false; };
@@ -287,17 +332,33 @@ bool future_ops(const serfsim* h, u32 after_tick) {       // any op scheduled at
   return !h->ops.empty() && h->ops.back().tick > after_tick;
 }
 
-bool ops_at(const serfsim* h, u32 t) {
-  auto it = std::lower_bound(h->ops.begin(), h->ops.end(), t, [](const HostOp& o, u32 tt) { return o.tick < tt; });
-  return it != h->ops.end() && it->tick == t;
+// The host operations of tick t: ops[begin, end) (ops is sorted by tick).
+struct OpRange { u32 begin, end; };
+OpRange ops_of_tick(const serfsim* h, u32 t) {
+  auto lo = std::lower_bound(h->ops.begin(), h->ops.end(), t, [](const HostOp& o, u32 tt) { return o.tick < tt; });
+  auto hi = std::upper_bound(lo, h->ops.end(), t, [](u32 tt, const HostOp& o) { return tt < o.tick; });
+  return {(u32)(lo - h->ops.begin()), (u32)(hi - h->ops.begin())};
 }
+bool ops_at(const serfsim* h, u32 t) { const OpRange r = ops_of_tick(h, t); return r.end > r.begin; }
 bool reap_tick(const serfsim* h, u32 t) { return h->cfg.reap_interval_ticks && ((t + 1) % h->cfg.reap_interval_ticks) == 0; }
-// Multi-slot production runs: does tick t run as per-view passes (SV_PASS, tick_kernel.cuh)?  Unsharded ticks without a host operation
-// or a reaper round.  (mode: the SERFSIM_SV mode it is asked for; check mode takes the same ticks to the general kernel)
-bool pass_tick(const serfsim* h, u32 t, u32 mode) {
-  const bool sleep_on = !h->no_skip && !h->byz_on;
-  return h->sv == mode && h->R > 1 && h->R < 32 && !h->cfg.trace && sleep_on && h->cfg.world_size == 1 && !ops_at(h, t) && !reap_tick(h, t) &&
-         t + 1 < CARRY_TICKS;
+bool pp_tick(const serfsim* h, u32 t) {         // an anti-entropy round follows tick t
+  const u32 pp = (u32)std::max(0, h->cfg.push_pull_interval_ticks);
+  return pp && (t + 1) % pp == 0;
+}
+
+// How tick t launches its membership kernels (SV_*, tick_kernel.cuh): the one place that decides it.  Multi-slot runs in production mode
+// (no trace, no SERFSIM_NO_SKIP, no injectors): unsharded ticks without a host operation or a reaper round run as per-view passes; sharded
+// ticks while exactly one subject has ever been down launch the general and the single-view kernel and the device decides (dual launch).
+// SERFSIM_SV=2 takes both to the general kernel in check mode.  Call it after the tick's down subjects are in ever_down.
+enum class TickRun { General, Passes, Check, Dual };
+TickRun tick_run(const serfsim* h, u32 t) {
+  if (!h->sw.sv || h->R < 2 || h->R >= 32 || h->cfg.trace || h->sw.no_skip || h->byz_on) return TickRun::General;
+  if (h->cfg.world_size > 1) {
+    if (__builtin_popcount(h->ever_down) != 1) return TickRun::General;
+    return h->sw.sv == 2 ? TickRun::Check : TickRun::Dual;
+  }
+  if (ops_at(h, t) || reap_tick(h, t) || t + 1 >= CARRY_TICKS) return TickRun::General;
+  return h->sw.sv == 2 ? TickRun::Check : TickRun::Passes;
 }
 // The passes of tick t + 1 choose their loads from their own views' counters of tick t (TickParams::view_kinds_prev) only if every
 // inbox write of tick t was a pass's: otherwise (general kernel — host operation, reaper round, trace mode, SERFSIM_SV=0/2 — anti-entropy
@@ -305,8 +366,226 @@ bool pass_tick(const serfsim* h, u32 t, u32 mode) {
 // tick's counters.  Ticks the host jumped over or the device skipped sent nothing: their zero rows are exact either way.  This is the
 // one place that decides it.
 bool view_kinds_valid(const serfsim* h, u32 t) {
-  const u32 pp = (u32)std::max(0, h->cfg.push_pull_interval_ticks);
-  return pass_tick(h, t, 1) && !(pp && (t + 1) % pp == 0);          // (injectors: pass_tick is false)
+  return tick_run(h, t) == TickRun::Passes && !pp_tick(h, t);          // (injectors: never passes)
+}
+
+// The planes as the single-slot kernel sees them: p with every per-slot plane starting at view s, on the single-slot kernel's grid.
+TickParams at_view(const serfsim* h, const TickParams& p, u32 s) {
+  TickParams q = p;
+  q.sv_wshift = s;
+  q.rec = p.rec + 2 * (size_t)s * h->stride; q.qword = p.qword + (size_t)s * h->stride;
+  q.inbox_rd = p.inbox_rd + (size_t)s * h->stride; q.inbox_wr = p.inbox_wr + (size_t)s * h->stride;
+  q.subj[0] = p.subj[s]; q.down_mask = (p.down_mask >> s) & 1u;
+  q.tiles_per_cta = (h->n_tiles + h->grid_sv - 1) / h->grid_sv;
+  return q;
+}
+
+// Timing events, created on first use: ev holds at least n.
+int grow_events(std::vector<cudaEvent_t>& ev, size_t n) {
+  while (ev.size() < n) { cudaEvent_t e; CU(cudaEventCreate(&e)); ev.push_back(e); }
+  return 0;
+}
+
+// The tracked user events' Lamport times as the cluster knows them: the origin's shard stamps an event, the other shards may not have it
+// yet, so each contributes the stamps of its own nodes' events and every rank gets the sum (a collective when sharded).  Stream idle.
+int ue_cluster_ltimes(serfsim* h, u32 lt[MAX_UEVENTS]) {
+  CU(cudaMemcpy(lt, h->d_ue_ltime, MAX_UEVENTS * sizeof(u32), cudaMemcpyDeviceToHost));
+  if (h->cfg.world_size > 1 && h->allreduce) {
+    u64 v[MAX_UEVENTS];
+    for (u32 e = 0; e < MAX_UEVENTS; ++e) v[e] = (((h->ue_injected >> e) & 1u) && h->ue_origin[e] - h->first < h->count) ? lt[e] : 0;
+    h->allreduce(h->comm_user, v, MAX_UEVENTS);
+    for (u32 e = 0; e < MAX_UEVENTS; ++e) lt[e] = (u32)v[e];
+  }
+  return 0;
+}
+
+// The summary kernel's output: [0] largest clock, [1] queued intents, [2 + 2s] / [3 + 2s] least / greatest status word of view s.
+int read_summary(serfsim* h, std::vector<u64>& out) {
+  const u32 nout = 2 + 2 * h->R;
+  std::vector<u64> init(nout, 0);
+  for (u32 s = 0; s < h->R; ++s) init[2 + 2 * s] = ~0ull;
+  out.resize(nout);
+  CU(cudaMemcpyAsync(h->d_scratch, init.data(), nout * 8, cudaMemcpyHostToDevice, h->stream));
+  launch_summary(h->d_rec, h->d_qword, h->d_node, h->count, h->stride, h->first, h->R, h->d_subj, h->d_scratch, h->stream);
+  CU(cudaMemcpyAsync(out.data(), h->d_scratch, nout * 8, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// The membership tick's block for tick t with host operations ops[ops.begin, ops.end); the other blocks take their shared fields from it.
+TickParams tick_params(const serfsim* h, u32 t, OpRange ops) {
+  TickParams p{};
+  p.n_local = h->count; p.first = h->first; p.n_global = h->N; p.R = h->R;
+  p.fanout = h->cfg.fanout; p.probe_every = h->cfg.probe_interval_ticks; p.tick = t;
+  p.down_mask = (~h->up_mask) & ((1u << h->R) - 1);
+  p.seed_lo = (u32)h->cfg.seed; p.seed_hi = (u32)(h->cfg.seed >> 32); p.ev_begin = ops.begin; p.ev_end = ops.end;
+  p.rules = h->rules;
+  for (u32 s = 0; s < h->R; ++s) p.subj[s] = h->subj[s];
+  p.rec = h->d_rec; p.qword = h->d_qword; p.inbox_rd = h->d_inbox[(t & 1) ^ 1]; p.inbox_wr = h->d_inbox[t & 1];
+  p.node_state = h->d_node; p.busy = h->d_busy; p.watch = h->d_watch; p.row_ptr = h->d_rowptr; p.col = h->d_col;
+  p.ev_node = h->d_ev_node; p.ev_op = h->d_ev_op; p.ev_slot = h->d_ev_slot;
+  p.row = h->d_trace + (size_t)t * 8;
+  p.kinds_prev = h->d_kinds + (size_t)t * 4;
+  p.kinds_cur = h->d_kinds + ((size_t)t + 1) * 4;
+  p.overflow = h->d_overflow;
+  p.hot_rd = h->d_hot[(t & 1) ^ 1]; p.hot_wr = h->d_hot[t & 1];
+  p.stage_col_bytes = h->stage_col_bytes;
+  p.reap_now = reap_tick(h, t) ? 1u : 0u;
+  p.tombstone_ticks = h->cfg.tombstone_timeout_ticks; p.reconnect_ticks = h->cfg.reconnect_timeout_ticks; p.intent_ticks = h->cfg.recent_intent_timeout_ticks;
+  p.stride = h->stride; p.n_tiles = h->n_tiles; p.tiles_per_cta = (h->n_tiles + h->grid - 1) / h->grid;
+  p.force_all = (h->cfg.trace != 0) || h->sw.no_skip || p.reap_now;
+  p.compact = h->sw.compact ? 1u : 0u;
+  p.dedup = h->sw.dedup ? 1u : 0u;
+  p.udeg = h->udeg; p.ahead = h->sw.ahead;
+  p.tile_due = h->d_tile_due; p.node_due = h->d_node_due; p.hot_static = h->d_hot_static; p.sched = h->d_sched;
+  p.sleep_on = (h->sw.no_skip || h->byz_on) ? 0u : 1u;          // injectors send every tick: the cluster never sleeps
+  p.pp_every = (u32)std::max(0, h->cfg.push_pull_interval_ticks); p.reap_every = h->cfg.reap_interval_ticks;
+  p.host_idle_until = h->d_pin_ctl + 2;
+  const bool sharded = h->cfg.world_size > 1;
+  const u32 xpar = h->xepoch & 1;
+  p.world = (u32)h->cfg.world_size; p.rank = (u32)h->cfg.rank; p.shard_size = h->shard_size; p.win_cap = h->win_cap;
+  p.win_data = h->d_peer_data[xpar]; p.send_count = h->d_send_count;
+  p.peer_ctrl = h->d_peer_ctrl; p.stamp = h->xepoch + 1; p.xpar = xpar; p.loopback = h->loopback ? 1u : 0u;
+  p.fuse_publish = (sharded && !h->byz_on && !h->sw.no_fuse) ? 1u : 0u;
+  p.shard_inv = (u32)(0x100000000ull / h->shard_size); p.xcap = p.world > 1 ? 392u / (p.world - 1) : 0u;     // XW_TOTAL = 392 (tick_kernel.cu)
+  if (h->gate_on) {                                // convergence gate: the first kernel of the tick evaluates the row of tick t-1
+    const u64* grow = sharded ? h->d_grow : h->d_trace;            // global rows: the device sums them when sharded
+    Gate& g = p.gate;
+    g.ctl = h->d_runctl; g.host_ctl = h->d_pin_ctl; g.prev_row = t > h->gate_first ? grow + (size_t)(t - 1) * 8 : nullptr; g.tick = t;
+    g.future_ops = (t > 0 && future_ops(h, t - 1)) ? 1u : 0u;
+    g.pp = p.pp_every; g.byz_on = h->byz_on ? 1u : 0u;
+  }
+  p.gate.evaluate = h->ue_table.n ? 0u : 1u;       // with user events on, their kernel is the tick's first
+  return p;
+}
+
+// The user-event tick: it needs the pre-operation up flags and op bits, so it runs first and evaluates the gate.
+void launch_user_events(serfsim* h, const TickParams& p) {
+  const u32 t = p.tick;
+  UeParams u{};
+  u.n_local = h->count; u.first = h->first; u.n_global = h->N; u.R = h->R; u.fanout = h->cfg.fanout; u.tick = t;
+  u.seed_lo = p.seed_lo; u.seed_hi = p.seed_hi; u.limit = h->rules.limit; u.ev_begin = p.ev_begin; u.ev_end = p.ev_end;
+  u.table = h->ue_table; u.state = h->d_ue_state; u.inbox_rd = h->d_ue_inbox[(t & 1) ^ 1]; u.inbox_wr = h->d_ue_inbox[t & 1];
+  u.ltime = h->d_ue_ltime; u.node_state = h->d_node; u.busy = h->d_busy; u.row_ptr = h->d_rowptr; u.col = h->d_col;
+  u.ev_node = h->d_ev_node; u.ev_op = h->d_ev_op; u.ev_slot = h->d_ev_slot;
+  u.row = p.row; u.totals = h->d_ue_totals; u.overflow = h->d_overflow; u.sched = h->d_sched;
+  u.world = p.world; u.rank = p.rank; u.shard_size = h->shard_size; u.win_cap = h->win_cap;
+  u.win_data = p.win_data; u.send_count = h->d_send_count;
+  u.gate = p.gate; u.gate.evaluate = 1u;
+  launch_uevent(u, h->cfg.trace != 0, h->stream);
+  h->last_launches++;
+}
+
+// The membership tick as tick_run decides it: the general kernel, per-view passes of the single-slot kernel, or the general kernel and
+// the single-view kernel.  p leaves with the fields the launch set (the anti-entropy round takes it as it is).
+void launch_membership(serfsim* h, TickParams& p) {
+  const u32 t = p.tick;
+  const TickRun run = tick_run(h, t);
+  if (run != TickRun::General) {
+    p.views_host = p.ev_end > p.ev_begin || p.reap_now ? 0xffffffffu : h->ever_down;   // a host operation or a reaper round visits every view
+    p.sv_mode = h->sw.sv == 2 ? SV_CHECK : SV_GENERAL;
+    p.sv_slot = h->ever_down ? (u32)__builtin_ctz(h->ever_down) : 0u; p.sv_R = h->R;
+  }
+  if (run == TickRun::Passes) {
+    p.sv_mode = SV_PASS; p.carry = h->d_carry;
+    p.tiles_per_cta = (h->n_tiles + h->grid_sv - 1) / h->grid_sv;
+    const bool own = t > 0 && view_kinds_valid(h, t - 1);
+    for (u32 s0 = 0; s0 < h->R; ++s0) {                  // ascending slot order: what the view loop carries from view to view travels through memory
+      TickParams q = at_view(h, p, s0);
+      q.gate.evaluate = s0 == 0 ? p.gate.evaluate : 0u; q.sv_slot = s0;
+      q.view_kinds_prev = own ? h->d_view_kinds + ((size_t)t * h->R + s0) * 4 : p.kinds_prev;
+      q.view_kinds_cur = h->d_view_kinds + (((size_t)t + 1) * h->R + s0) * 4;
+      launch_tick_pass(q, h->grid_sv, h->stream);
+      h->last_launches++;
+    }
+  } else {
+    launch_tick(p, h->cfg.trace != 0, h->grid, h->ctas_per_sm, h->sw.tma_sync, h->stream);
+    h->last_launches++;
+  }
+  if (run == TickRun::Dual) {
+    TickParams q = at_view(h, p, p.sv_slot);
+    q.sv_mode = SV_SINGLE; q.gate.evaluate = 0u;
+    launch_tick_single_view(q, h->grid_sv, h->stream);
+    h->last_launches++;
+  }
+}
+
+// Stale entries of this shard's injectors (before the exchange: peers in other shards get window entries).
+void launch_injectors(serfsim* h, const TickParams& p) {
+  const u32 t = p.tick;
+  ByzParams b{};
+  b.n_byz = h->byz_n; b.first = h->first; b.R = h->R; b.stride = h->stride; b.fanout = h->cfg.fanout; b.tick = t;
+  b.seed_lo = p.seed_lo; b.seed_hi = p.seed_hi; b.delta = h->byz_delta; b.ids = h->d_byz_ids; b.rec = h->d_rec; b.node_state = h->d_node;
+  b.row_ptr = h->d_rowptr; b.col = h->d_col; b.inbox_wr = h->d_inbox[t & 1]; b.hot_wr = h->d_hot[t & 1]; b.kinds_cur = p.kinds_cur;
+  b.anomaly = h->d_anomaly; b.totals = h->d_byz_totals;
+  b.n_local = h->count; b.world = p.world; b.rank = p.rank; b.shard_size = h->shard_size; b.win_cap = h->win_cap;
+  b.win_data = p.win_data; b.send_count = h->d_send_count; b.overflow = h->d_overflow; b.gate = p.gate.ctl;
+  launch_byz(b, h->stream);
+  h->last_launches++;
+}
+
+// The exchange of a sharded tick.  No host round trip: publish (counts + flag into every peer's control block) and drain (waits for the
+// peers' flags of this exchange) are ordinary kernels on the same stream.
+void launch_exchange(serfsim* h, const TickParams& p) {
+  const u32 t = p.tick, xpar = p.xpar;
+  PublishParams pb{};
+  pb.world = p.world; pb.rank = p.rank; pb.stamp = p.stamp; pb.xpar = xpar; pb.send_count = h->d_send_count; pb.peer_ctrl = h->d_peer_ctrl;
+  pb.row = p.row; pb.gate = p.gate.ctl; pb.sched = h->d_sched; pb.loopback = p.loopback;
+  if (!p.fuse_publish) { launch_publish(pb, h->stream); h->last_launches++; }
+  DrainParams d{};
+  d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.world; d.rank = p.rank; d.win_cap = h->win_cap; d.stamp = p.stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
+  d.win_data = h->d_win_data[xpar]; d.ctrl = h->d_ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
+  d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = h->d_peer_anomaly;
+  d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->d_ue_inbox[t & 1] : nullptr; d.ue_ltime = h->d_ue_ltime;
+  d.my_row = p.row; d.grow = h->d_grow + (size_t)t * 8; d.gate = p.gate.ctl;
+  d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(h->d_ctrl) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
+  d.sched = h->d_sched; d.sched_rw = h->d_sched; d.host_idle_until = h->d_pin_ctl + 2; d.tick = t; d.sleep_on = p.sleep_on;
+  launch_drain(d, h->stream);
+  h->last_launches += 1;
+  h->xepoch++;
+}
+
+// Anti-entropy round on a snapshot of the end-of-tick state (only this node's own records are written); p: as the membership tick left it.
+int anti_entropy_round(serfsim* h, TickParams p) {
+  const u32 t = p.tick;
+  const size_t rb = (size_t)h->R * h->stride * 32, nb = (size_t)h->stride * 8;
+  if (!h->d_snap_rec) { CU(cudaMalloc(&h->d_snap_rec, rb)); CU(cudaMalloc(&h->d_snap_node, nb)); }
+  CU(cudaMemcpyAsync(h->d_snap_rec, h->d_rec, rb, cudaMemcpyDeviceToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_snap_node, h->d_node, nb, cudaMemcpyDeviceToDevice, h->stream));
+  if (h->ue_table.n) {
+    CU(cudaMemcpyAsync(h->d_ue_snap, h->d_ue_state, (size_t)h->stride * 16, cudaMemcpyDeviceToDevice, h->stream));
+    p.ue_table = h->ue_table; p.ue_state = h->d_ue_state; p.ue_snap = h->d_ue_snap; p.ue_snap_peer = h->d_peer_ue_snap;
+    p.ue_ltime = h->d_ue_ltime; p.ue_totals = h->d_ue_totals;
+  }
+  if (h->cfg.world_size > 1) {
+    // partners may live on other GPUs: their snapshots are read through the peer mappings.  Rounds are rare (every
+    // push_pull_interval ticks) and always the first tick of a convergence chunk, so two host barriers are affordable:
+    // every rank has taken its snapshot before anyone reads, everyone has read before anyone moves on.
+    p.snap_rec_peer = h->d_peer_snap_rec; p.snap_node_peer = h->d_peer_snap_node;
+    CU(cudaStreamSynchronize(h->stream));
+    h->barrier(h->comm_user);
+    if (h->ue_table.n) {
+      // A partner in another shard may hold events this shard has never received, so their Lamport times are not in the
+      // local table yet (a shard learns them from the first window entry of the event).  The replay needs them: every rank
+      // installs the cluster's times before the round.
+      u32 lt[MAX_UEVENTS];
+      if (int rc = ue_cluster_ltimes(h, lt)) return rc;
+      CU(cudaMemcpy(h->d_ue_ltime, lt, sizeof(lt), cudaMemcpyHostToDevice));
+    }
+    launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
+    CU(cudaStreamSynchronize(h->stream));
+    h->barrier(h->comm_user);
+    // the round changed this rank's row (changed / pending / hash) after the drain kernel summed the rows: redo the sum through
+    // the host hook — the host is in the loop here anyway (two barriers), and rounds are rare
+    u64 row[8];
+    CU(cudaMemcpy(row, h->d_trace + (size_t)t * 8, sizeof(row), cudaMemcpyDeviceToHost));
+    h->allreduce(h->comm_user, row, 8);
+    CU(cudaMemcpy(h->d_grow + (size_t)t * 8, row, sizeof(row), cudaMemcpyHostToDevice));
+  } else {
+    launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
+  }
+  h->last_launches++;
+  return 0;
 }
 
 // Launch n ticks on the stream (no synchronisation).
@@ -318,66 +597,23 @@ int launch_ticks(serfsim* h, u32 n) {
   rc = ensure_trace(h, h->tick + n + 1);
   if (rc) return rc;
   if (!h->timing_open) { CU(cudaEventRecord(h->ev0, h->stream)); h->timing_open = true; h->last_launches = 0; h->launch_log.clear(); h->launch_log_first = h->tick; }
-  const bool sharded = h->cfg.world_size > 1;
-  const u64* grow = sharded ? h->d_grow : h->d_trace;            // global rows: the device sums them when sharded
   for (u32 i = 0; i < n; ++i) {
     const u32 t = h->tick;
     const u64 launches_before = h->last_launches;
-    auto lo = std::lower_bound(h->ops.begin(), h->ops.end(), t, [](const HostOp& o, u32 tt) { return o.tick < tt; });
-    auto hi = std::upper_bound(h->ops.begin(), h->ops.end(), t, [](u32 tt, const HostOp& o) { return tt < o.tick; });
-    const u32 eb = (u32)(lo - h->ops.begin()), ee = (u32)(hi - h->ops.begin());
-    for (auto it = lo; it != hi; ++it) {          // ground truth the SWIM probe observes (after this tick's ops)
-      const int s = slot_of(h, it->node);
-      if (s >= 0) { if (it->op == SERFSIM_OP_FAIL) h->up_mask &= ~(1u << s); if (it->op == SERFSIM_OP_REJOIN) h->up_mask |= (1u << s); }
+    const OpRange ops = ops_of_tick(h, t);
+    for (u32 k = ops.begin; k < ops.end; ++k) {     // ground truth the SWIM probe observes (after this tick's ops)
+      const HostOp& o = h->ops[k];
+      const int s = slot_of(h, o.node);
+      if (s >= 0) { if (o.op == SERFSIM_OP_FAIL) h->up_mask &= ~(1u << s); if (o.op == SERFSIM_OP_REJOIN) h->up_mask |= (1u << s); }
     }
-    if (ee > eb) { launch_mark_events(h->d_busy, h->d_hot[(t & 1) ^ 1], h->d_ev_node, eb, ee, h->first, h->count, h->stream); h->last_launches++; }
-    TickParams p{};
-    p.n_local = h->count; p.first = h->first; p.n_global = h->N; p.R = h->R;
-    p.fanout = h->cfg.fanout; p.probe_every = h->cfg.probe_interval_ticks; p.tick = t;
-    p.down_mask = (~h->up_mask) & ((1u << h->R) - 1);
+    if (ops.end > ops.begin) { launch_mark_events(h->d_busy, h->d_hot[(t & 1) ^ 1], h->d_ev_node, ops.begin, ops.end, h->first, h->count, h->stream); h->last_launches++; }
+    TickParams p = tick_params(h, t, ops);
     h->ever_down |= p.down_mask;
-    p.seed_lo = (u32)h->cfg.seed; p.seed_hi = (u32)(h->cfg.seed >> 32); p.ev_begin = eb; p.ev_end = ee;
-    p.rules = h->rules;
-    for (u32 s = 0; s < h->R; ++s) p.subj[s] = h->subj[s];
-    p.rec = h->d_rec; p.qword = h->d_qword; p.inbox_rd = h->d_inbox[(t & 1) ^ 1]; p.inbox_wr = h->d_inbox[t & 1];
-    p.node_state = h->d_node; p.busy = h->d_busy; p.watch = h->d_watch; p.row_ptr = h->d_rowptr; p.col = h->d_col;
-    p.ev_node = h->d_ev_node; p.ev_op = h->d_ev_op; p.ev_slot = h->d_ev_slot;
-    p.row = h->d_trace + (size_t)t * 8;
-    p.kinds_prev = h->d_kinds + (size_t)t * 4;
-    p.kinds_cur = h->d_kinds + ((size_t)t + 1) * 4;
-    p.overflow = h->d_overflow;
-    p.hot_rd = h->d_hot[(t & 1) ^ 1]; p.hot_wr = h->d_hot[t & 1];
-    p.stage_col_bytes = h->stage_col_bytes;
-    p.reap_now = reap_tick(h, t) ? 1u : 0u;
-    p.tombstone_ticks = h->cfg.tombstone_timeout_ticks; p.reconnect_ticks = h->cfg.reconnect_timeout_ticks; p.intent_ticks = h->cfg.recent_intent_timeout_ticks;
-    p.stride = h->stride; p.n_tiles = h->n_tiles; p.tiles_per_cta = (h->n_tiles + h->grid - 1) / h->grid;
-    p.force_all = (h->cfg.trace != 0) || h->no_skip || p.reap_now;
-    p.compact = h->compact ? 1u : 0u;
-    p.dedup = h->dedup ? 1u : 0u;
-    p.udeg = h->udeg; p.ahead = h->ahead;
-    p.tile_due = h->d_tile_due; p.node_due = h->d_node_due; p.hot_static = h->d_hot_static; p.sched = h->d_sched;
-    p.sleep_on = (h->no_skip || h->byz_on) ? 0u : 1u;          // injectors send every tick: the cluster never sleeps
-    p.pp_every = (u32)std::max(0, h->cfg.push_pull_interval_ticks); p.reap_every = h->cfg.reap_interval_ticks;
-    p.host_idle_until = h->d_pin_ctl + 2;
-    const u32 xpar = h->xepoch & 1;
-    p.world = (u32)h->cfg.world_size; p.rank = (u32)h->cfg.rank; p.shard_size = h->shard_size; p.win_cap = h->win_cap;
-    p.win_data = h->d_peer_data[xpar]; p.send_count = h->d_send_count;
-    p.peer_ctrl = h->d_peer_ctrl; p.stamp = h->xepoch + 1; p.xpar = xpar; p.loopback = h->loopback ? 1u : 0u;
-    p.fuse_publish = (sharded && !h->byz_on && !getenv("SERFSIM_NO_FUSE")) ? 1u : 0u;
-    p.shard_inv = (u32)(0x100000000ull / h->shard_size); p.xcap = p.world > 1 ? 392u / (p.world - 1) : 0u;     // XW_TOTAL = 392 (tick_kernel.cu)
-    Gate gate{};                                   // convergence gate: the first kernel of the tick evaluates the row of tick t-1
-    if (h->gate_on) {
-      gate.ctl = h->d_runctl; gate.host_ctl = h->d_pin_ctl; gate.prev_row = t > h->gate_first ? grow + (size_t)(t - 1) * 8 : nullptr; gate.tick = t;
-      gate.future_ops = (t > 0 && future_ops(h, t - 1)) ? 1u : 0u;
-      gate.pp = (u32)std::max(0, h->cfg.push_pull_interval_ticks); gate.byz_on = h->byz_on ? 1u : 0u;
-    }
-    const u32* gate_word = h->gate_on ? h->d_runctl : nullptr;
-    p.gate = gate; p.gate.evaluate = h->ue_table.n ? 0u : 1u;
     if (h->tick_timing) {
-      while (h->tick_ev.size() < 2 * ((size_t)t + 1)) { cudaEvent_t e; CU(cudaEventCreate(&e)); h->tick_ev.push_back(e); }
+      if ((rc = grow_events(h->tick_ev, 2 * ((size_t)t + 1)))) return rc;
       CU(cudaEventRecord(h->tick_ev[2 * (size_t)t], h->stream));
     }
-    if (h->l2_window && h->l2_window_max) {
+    if (h->sw.l2_window && h->l2_window_max) {
       cudaStreamAttrValue av{};
       const size_t bytes = (size_t)3 * h->R * h->stride * sizeof(u32);
       av.accessPolicyWindow.base_ptr = h->d_inbox[t & 1];
@@ -387,142 +623,17 @@ int launch_ticks(serfsim* h, u32 n) {
       av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
       CU(cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &av));
     }
-    if (h->ue_table.n) {                       // user-event tick: needs the pre-operation up flags and op bits, so it runs first
-      UeParams u{};
-      u.n_local = h->count; u.first = h->first; u.n_global = h->N; u.R = h->R; u.fanout = h->cfg.fanout; u.tick = t;
-      u.seed_lo = p.seed_lo; u.seed_hi = p.seed_hi; u.limit = h->rules.limit; u.ev_begin = eb; u.ev_end = ee;
-      u.table = h->ue_table; u.state = h->d_ue_state; u.inbox_rd = h->d_ue_inbox[(t & 1) ^ 1]; u.inbox_wr = h->d_ue_inbox[t & 1];
-      u.ltime = h->d_ue_ltime; u.node_state = h->d_node; u.busy = h->d_busy; u.row_ptr = h->d_rowptr; u.col = h->d_col;
-      u.ev_node = h->d_ev_node; u.ev_op = h->d_ev_op; u.ev_slot = h->d_ev_slot;
-      u.row = p.row; u.totals = h->d_ue_totals; u.overflow = h->d_overflow; u.sched = h->d_sched;
-      u.world = (u32)h->cfg.world_size; u.rank = (u32)h->cfg.rank; u.shard_size = h->shard_size; u.win_cap = h->win_cap;
-      u.win_data = h->d_peer_data[h->xepoch & 1]; u.send_count = h->d_send_count;
-      u.gate = gate; u.gate.evaluate = 1u;
-      launch_uevent(u, h->cfg.trace != 0, h->stream);
-      h->last_launches++;
-    }
-    // Multi-slot runs in production mode (SV_*, tick_kernel.cuh).  Unsharded: ticks without a host operation or a reaper round run as
-    // per-view passes of the single-slot kernel.  Sharded: while exactly one subject has ever been down, the general kernel and the
-    // single-view kernel are both launched and the device decides.
-    const bool sv_ok = h->sv && h->R > 1 && h->R < 32 && !h->cfg.trace && p.sleep_on && !h->byz_on;
-    const bool passes = pass_tick(h, t, 1), check = pass_tick(h, t, 2);
-    const bool dual = sv_ok && sharded && __builtin_popcount(h->ever_down) == 1;
-    if (passes || check || dual) {
-      const bool all = ee > eb || p.reap_now;                 // a host operation or a reaper round visits every view
-      p.views_host = all ? 0xffffffffu : h->ever_down;
-      p.sv_mode = h->sv == 2 ? SV_CHECK : SV_GENERAL;
-      p.sv_slot = h->ever_down ? (u32)__builtin_ctz(h->ever_down) : 0u; p.sv_R = h->R;
-    }
-    if (passes) {
-      p.sv_mode = SV_PASS; p.carry = h->d_carry;
-      p.tiles_per_cta = (h->n_tiles + h->grid_sv - 1) / h->grid_sv;
-      const bool own = t > 0 && view_kinds_valid(h, t - 1);
-      for (u32 s0 = 0; s0 < h->R; ++s0) {                  // ascending slot order: what the view loop carries from view to view travels through memory
-        TickParams q = p;                                  // the planes as the single-slot kernel sees them: they start at view s0
-        q.gate.evaluate = s0 == 0 ? p.gate.evaluate : 0u; q.sv_wshift = s0; q.sv_slot = s0;
-        q.view_kinds_prev = own ? h->d_view_kinds + ((size_t)t * h->R + s0) * 4 : p.kinds_prev;
-        q.view_kinds_cur = h->d_view_kinds + (((size_t)t + 1) * h->R + s0) * 4;
-        q.rec = p.rec + 2 * (size_t)s0 * h->stride; q.qword = p.qword + (size_t)s0 * h->stride;
-        q.inbox_rd = p.inbox_rd + (size_t)s0 * h->stride; q.inbox_wr = p.inbox_wr + (size_t)s0 * h->stride;
-        q.subj[0] = p.subj[s0]; q.down_mask = (p.down_mask >> s0) & 1u;
-        launch_tick_pass(q, h->grid_sv, h->stream);
-        h->last_launches++;
-      }
-    } else {
-      launch_tick(p, h->cfg.trace != 0, h->grid, h->stream);
-      h->last_launches++;
-    }
-    if (dual && h->sv == 1) {
-      TickParams q = p;                                    // the planes as the single-slot kernel sees them: they start at view sv_slot
-      const u32 s0 = p.sv_slot;
-      q.sv_mode = SV_SINGLE; q.gate.evaluate = 0u; q.sv_wshift = s0;
-      q.rec = p.rec + 2 * (size_t)s0 * h->stride; q.qword = p.qword + (size_t)s0 * h->stride;
-      q.inbox_rd = p.inbox_rd + (size_t)s0 * h->stride; q.inbox_wr = p.inbox_wr + (size_t)s0 * h->stride;
-      q.subj[0] = p.subj[s0]; q.down_mask = (p.down_mask >> s0) & 1u;
-      q.tiles_per_cta = (h->n_tiles + h->grid_sv - 1) / h->grid_sv;
-      launch_tick_single_view(q, h->grid_sv, h->stream);
-      h->last_launches++;
-    }
-    if (h->byz_n) {                            // stale entries of this shard's injectors (before the exchange: peers in other shards get window entries)
-      ByzParams b{};
-      b.n_byz = h->byz_n; b.first = h->first; b.R = h->R; b.stride = h->stride; b.fanout = h->cfg.fanout; b.tick = t;
-      b.seed_lo = p.seed_lo; b.seed_hi = p.seed_hi; b.delta = h->byz_delta; b.ids = h->d_byz_ids; b.rec = h->d_rec; b.node_state = h->d_node;
-      b.row_ptr = h->d_rowptr; b.col = h->d_col; b.inbox_wr = h->d_inbox[t & 1]; b.hot_wr = h->d_hot[t & 1]; b.kinds_cur = p.kinds_cur;
-      b.anomaly = h->d_anomaly; b.totals = h->d_byz_totals;
-      b.n_local = h->count; b.world = p.world; b.rank = p.rank; b.shard_size = h->shard_size; b.win_cap = h->win_cap;
-      b.win_data = p.win_data; b.send_count = h->d_send_count; b.overflow = h->d_overflow; b.gate = gate_word;
-      launch_byz(b, h->stream);
-      h->last_launches++;
-    }
-    if (h->tick_timing && h->cfg.world_size > 1) {
-      while (h->mid_ev.size() < (size_t)t + 1) { cudaEvent_t e; CU(cudaEventCreate(&e)); h->mid_ev.push_back(e); }
-      CU(cudaEventRecord(h->mid_ev[t], h->stream));
-    }
+    if (h->ue_table.n) launch_user_events(h, p);
+    launch_membership(h, p);
+    if (h->byz_n) launch_injectors(h, p);
     if (h->cfg.world_size > 1) {
-      // No host round trip: publish (counts + flag into every peer's control block) and drain (waits for the
-      // peers' flags of this exchange) are ordinary kernels on the same stream.
-      const u32 stamp = h->xepoch + 1;
-      PublishParams pb{};
-      pb.world = p.world; pb.rank = p.rank; pb.stamp = stamp; pb.xpar = xpar; pb.send_count = h->d_send_count; pb.peer_ctrl = h->d_peer_ctrl;
-      pb.row = p.row; pb.gate = gate_word; pb.sched = h->d_sched; pb.loopback = h->loopback ? 1u : 0u;
-      if (!p.fuse_publish) { launch_publish(pb, h->stream); h->last_launches++; }
-      DrainParams d{};
-      d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.world; d.rank = p.rank; d.win_cap = h->win_cap; d.stamp = stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
-      d.win_data = h->d_win_data[xpar]; d.ctrl = h->d_ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = h->d_kinds + ((size_t)t + 1) * 4; d.overflow = h->d_overflow;
-      d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = h->d_peer_anomaly;
-      d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->d_ue_inbox[t & 1] : nullptr; d.ue_ltime = h->d_ue_ltime;
-      d.my_row = p.row; d.grow = h->d_grow + (size_t)t * 8; d.gate = gate_word;
-      d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(h->d_ctrl) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
-      d.sched = h->d_sched; d.sched_rw = h->d_sched; d.host_idle_until = h->d_pin_ctl + 2; d.tick = t; d.sleep_on = p.sleep_on;
-      launch_drain(d, h->stream);
-      h->last_launches += 1;
-      h->xepoch++;
-    }
-    const u32 pp = (u32)std::max(0, h->cfg.push_pull_interval_ticks);
-    if (pp && (t + 1) % pp == 0) {
-      // anti-entropy round on a snapshot of the end-of-tick state (only this node's own records are written)
-      const size_t rb = (size_t)h->R * h->stride * 32, nb = (size_t)h->stride * 8;
-      if (!h->d_snap_rec) { CU(cudaMalloc(&h->d_snap_rec, rb)); CU(cudaMalloc(&h->d_snap_node, nb)); }
-      CU(cudaMemcpyAsync(h->d_snap_rec, h->d_rec, rb, cudaMemcpyDeviceToDevice, h->stream));
-      CU(cudaMemcpyAsync(h->d_snap_node, h->d_node, nb, cudaMemcpyDeviceToDevice, h->stream));
-      if (h->ue_table.n) {
-        CU(cudaMemcpyAsync(h->d_ue_snap, h->d_ue_state, (size_t)h->stride * 16, cudaMemcpyDeviceToDevice, h->stream));
-        p.ue_table = h->ue_table; p.ue_state = h->d_ue_state; p.ue_snap = h->d_ue_snap; p.ue_snap_peer = h->d_peer_ue_snap;
-        p.ue_ltime = h->d_ue_ltime; p.ue_totals = h->d_ue_totals;
+      if (h->tick_timing) {
+        if ((rc = grow_events(h->mid_ev, (size_t)t + 1))) return rc;
+        CU(cudaEventRecord(h->mid_ev[t], h->stream));
       }
-      if (h->cfg.world_size > 1) {
-        // partners may live on other GPUs: their snapshots are read through the peer mappings.  Rounds are rare (every
-        // push_pull_interval ticks) and always the first tick of a convergence chunk, so two host barriers are affordable:
-        // every rank has taken its snapshot before anyone reads, everyone has read before anyone moves on.
-        p.snap_rec_peer = h->d_peer_snap_rec; p.snap_node_peer = h->d_peer_snap_node;
-        CU(cudaStreamSynchronize(h->stream));
-        h->barrier(h->comm_user);
-        if (h->ue_table.n) {
-          // A partner in another shard may hold events this shard has never received, so their Lamport times are not in the
-          // local table yet (a shard learns them from the first window entry of the event).  The replay needs them: the
-          // origin's shard contributes its stamp, the others 0, and every rank installs the sum before the round.
-          u32 lt[MAX_UEVENTS];
-          u64 v[MAX_UEVENTS];
-          CU(cudaMemcpy(lt, h->d_ue_ltime, sizeof(lt), cudaMemcpyDeviceToHost));
-          for (u32 e = 0; e < MAX_UEVENTS; ++e) v[e] = (((h->ue_injected >> e) & 1u) && h->ue_origin[e] - h->first < h->count) ? lt[e] : 0;
-          h->allreduce(h->comm_user, v, MAX_UEVENTS);
-          for (u32 e = 0; e < MAX_UEVENTS; ++e) lt[e] = (u32)v[e];
-          CU(cudaMemcpy(h->d_ue_ltime, lt, sizeof(lt), cudaMemcpyHostToDevice));
-        }
-        launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
-        CU(cudaStreamSynchronize(h->stream));
-        h->barrier(h->comm_user);
-        // the round changed this rank's row (changed / pending / hash) after the drain kernel summed the rows: redo the sum through
-        // the host hook — the host is in the loop here anyway (two barriers), and rounds are rare
-        u64 row[8];
-        CU(cudaMemcpy(row, h->d_trace + (size_t)t * 8, sizeof(row), cudaMemcpyDeviceToHost));
-        h->allreduce(h->comm_user, row, 8);
-        CU(cudaMemcpy(h->d_grow + (size_t)t * 8, row, sizeof(row), cudaMemcpyHostToDevice));
-      } else {
-        launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
-      }
-      h->last_launches++;
+      launch_exchange(h, p);
     }
+    if (pp_tick(h, t) && (rc = anti_entropy_round(h, p))) return rc;
     if (h->tick_timing) CU(cudaEventRecord(h->tick_ev[2 * (size_t)t + 1], h->stream));
     h->launch_log.push_back((u32)(h->last_launches - launches_before));
     h->tick++;
@@ -546,13 +657,7 @@ int check_overflow(serfsim* h) {
     // Cluster runs need one Lamport time per ring slot: the packed event record derives a slot's ltime from the events in it.
     // (Two tracked events 512·k apart would alias — the quirk itself is kept in ue_handle and pinned by the handler tests.)
     u32 lt[MAX_UEVENTS];
-    CU(cudaMemcpy(lt, h->d_ue_ltime, sizeof(lt), cudaMemcpyDeviceToHost));
-    if (h->cfg.world_size > 1 && h->allreduce) {           // the origin's shard holds the stamp; the others may not have seen it yet
-      u64 v[MAX_UEVENTS];
-      for (u32 e = 0; e < MAX_UEVENTS; ++e) v[e] = (((h->ue_injected >> e) & 1u) && h->ue_origin[e] - h->first < h->count) ? lt[e] : 0;
-      h->allreduce(h->comm_user, v, MAX_UEVENTS);
-      for (u32 e = 0; e < MAX_UEVENTS; ++e) lt[e] = (u32)v[e];
-    }
+    if (int rc = ue_cluster_ltimes(h, lt)) return rc;
     for (u32 a = 0; a < h->ue_table.n; ++a)
       for (u32 b = a + 1; b < h->ue_table.n; ++b) {
         const bool fa = ((h->ue_injected >> a) & 1u) && h->ue_fire_tick[a] < h->tick, fb = ((h->ue_injected >> b) & 1u) && h->ue_fire_tick[b] < h->tick;
@@ -582,13 +687,8 @@ int pull_rows(serfsim* h) {                     // bring rows [rows.size(), tick
 
 int fire_events(serfsim* h) {
   if (!h->cb) return 0;
-  const u32 nout = 2 + 2 * h->R;
-  std::vector<u64> init(nout, 0), out(nout);
-  for (u32 s = 0; s < h->R; ++s) init[2 + 2 * s] = ~0ull;
-  CU(cudaMemcpyAsync(h->d_scratch, init.data(), nout * 8, cudaMemcpyHostToDevice, h->stream));
-  launch_summary(h->d_rec, h->d_qword, h->d_node, h->count, h->stride, h->first, h->R, h->d_subj, h->d_scratch, h->stream);
-  CU(cudaMemcpyAsync(out.data(), h->d_scratch, nout * 8, cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
+  std::vector<u64> out;
+  if (int rc = read_summary(h, out)) return rc;
   for (u32 type = 0; type < 3; ++type) {
     std::vector<u32> ids;
     for (u32 s = 0; s < h->R; ++s) {
@@ -670,7 +770,7 @@ void free_all(serfsim* h) {
   cudaFree(h->d_hot[0]); cudaFree(h->d_hot[1]); cudaFree(h->d_busy); cudaFree(h->d_watch); cudaFree(h->d_snap_rec); cudaFree(h->d_snap_node); cudaFree(h->d_peer_snap_rec); cudaFree(h->d_peer_snap_node);
   cudaFree(h->d_qword);
   cudaFree(h->d_rec); cudaFree(h->d_inbox[0]); cudaFree(h->d_inbox[1]); cudaFree(h->d_node); cudaFree(h->d_rowptr); cudaFree(h->d_col);
-  cudaFree(h->d_ev_node); cudaFree(h->d_ev_op); cudaFree(h->d_ev_slot); cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds); cudaFree(h->d_ones);
+  cudaFree(h->d_ev_node); cudaFree(h->d_ev_op); cudaFree(h->d_ev_slot); cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds);
   if (h->pin_overflow) cudaFreeHost(h->pin_overflow);
   cudaFree(h->d_subj); cudaFree(h->d_scratch); cudaFree(h->d_stage);
   cudaFree(h->d_byz_ids); cudaFree(h->d_anomaly); cudaFree(h->d_byz_totals); cudaFree(h->d_peer_anomaly);
@@ -687,6 +787,17 @@ void free_all(serfsim* h) {
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
+}
+
+// A peer's exported buffer mapped into this process (unmapped by free_all).
+template <class T>
+int ipc_open(serfsim* h, const cudaIpcMemHandle_t& handle, const char* what, T** out) {
+  void* ptr = nullptr;
+  const cudaError_t e = cudaIpcOpenMemHandle(&ptr, handle, cudaIpcMemLazyEnablePeerAccess);
+  if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(") + what + "): " + cudaGetErrorString(e));
+  h->ipc_opened.push_back(ptr);
+  *out = (T*)ptr;
+  return 0;
 }
 
 int getter(serfsim* h, u32 slot, int what, void* out, size_t elem) {
@@ -814,41 +925,29 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   CUB(cudaHostAlloc(&h->pin_ctl, 4 * sizeof(u32), cudaHostAllocMapped));
   CUB(cudaHostGetDevicePointer(&h->d_pin_ctl, h->pin_ctl, 0));
   h->pin_ctl[0] = h->pin_ctl[1] = h->pin_ctl[2] = h->pin_ctl[3] = 0;
-  CUB(cudaMalloc(&h->d_ones, 16));
-  const u32 ones[4] = {0x40000000u, 0x40000000u, 0x40000000u, 1u};   // multi-GPU: every inbox plane may hold entries, every tick is dense
-  CUB(cudaMemcpy(h->d_ones, ones, 16, cudaMemcpyHostToDevice));
   CUB(cudaMemcpy(h->d_subj, h->subj.data(), h->R * 4, cudaMemcpyHostToDevice));
-  {
-    const char* e = getenv("SERFSIM_MINB");
-    h->ctas_per_sm = (h->R == 1) ? ((e && atoi(e) == 5) ? 5 : (cfg->world_size > 1 ? tick_ctas_per_sm_r1s() : tick_ctas_per_sm_r1())) : tick_ctas_per_sm_rn();
-  }
-  h->grid = tick_grid_size(h->count, h->ctas_per_sm);
-  h->grid_sv = tick_grid_size(h->count, cfg->world_size > 1 ? tick_ctas_per_sm_r1s() : tick_ctas_per_sm_r1());
+  h->sw = read_switches();
+  cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, dev);
+  if (h->sms <= 0) h->sms = 132;
+  const int ctas_r1 = cfg->world_size > 1 ? tick_ctas_per_sm_r1s() : tick_ctas_per_sm_r1();
+  h->ctas_per_sm = h->R > 1 ? tick_ctas_per_sm_rn() : h->sw.minb5 ? 5 : ctas_r1;
+  h->grid = tick_grid_size(h->count, h->ctas_per_sm, h->sms, h->sw.gridmul);
+  h->grid_sv = tick_grid_size(h->count, ctas_r1, h->sms, h->sw.gridmul);
   {
     // L2 set-aside for persisting (evict_last) lines: the randomly addressed inbox planes live there
     int max_persist = 0, max_window = 0;
     cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev);
     cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, dev);
     h->l2_persist_max = (size_t)max_persist; h->l2_window_max = (size_t)max_window;
-    int want = 0;        // off by default: a carve-out takes L2 away from the streamed planes and the inbox alike
-    if (const char* e = getenv("SERFSIM_L2_PERSIST")) want = atoi(e);
-    if (want && max_persist > 0) cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)max_persist);
-    if (const char* e = getenv("SERFSIM_L2_WINDOW")) h->l2_window = atoi(e) != 0;
-    if (getenv("SERFSIM_VERBOSE")) fprintf(stderr, "serfsim: L2 persisting max %d B, window max %d B, persist %d window %d\n", max_persist, max_window, want, (int)h->l2_window);
+    if (h->sw.l2_persist && max_persist > 0) cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)max_persist);
+    if (h->sw.verbose) fprintf(stderr, "serfsim: L2 persisting max %d B, window max %d B, persist %d window %d\n", max_persist, max_window, h->sw.l2_persist, (int)h->sw.l2_window);
   }
-  if (const char* e = getenv("SERFSIM_NO_SKIP")) h->no_skip = atoi(e) != 0;
-  if (const char* e = getenv("SERFSIM_COMPACT")) h->compact = atoi(e) != 0;
-  if (const char* e = getenv("SERFSIM_DEDUP")) h->dedup = atoi(e) != 0;
-  if (const char* e = getenv("SERFSIM_AHEAD")) h->ahead = (u32)std::min(2, std::max(0, atoi(e)));
-  if (const char* e = getenv("SERFSIM_SV")) h->sv = (u32)std::min(2, std::max(0, atoi(e)));
   if (cfg->world_size > 1) {
     // receive windows: one segment per peer; expected entries per tick and pair ≈ shard · fanout · R · kinds / world
     if (cfg->world_size > 8) return bail(fail(SERFSIM_E_INVAL, "world_size > 8"));
-    double factor = 1.25;
-    if (const char* e = getenv("SERFSIM_WIN_FACTOR")) factor = atof(e);
     // … plus the entries the warps of the tick kernel reserve ahead and do not fill (flush_xwarp: at most XW_RESERVE_MAX = 128 per warp and peer)
-    const double pad = (double)std::max(tick_grid_size(h->count, h->ctas_per_sm), h->grid_sv) * 8.0 * 160.0;   // (the single-view kernel of a multi-slot run has the larger grid)
-    double cap = (double)h->shard_size * cfg->fanout * h->R * 3.0 * factor / cfg->world_size + 4096.0 + pad;
+    const double pad = (double)std::max(h->grid, h->grid_sv) * 8.0 * 160.0;   // (the single-view kernel of a multi-slot run has the larger grid)
+    double cap = (double)h->shard_size * cfg->fanout * h->R * 3.0 * h->sw.win_factor / cfg->world_size + 4096.0 + pad;
     h->win_cap = (u32)std::min(cap, 4.0e9);
     h->win_cap_base = h->win_cap;
     for (int par = 0; par < 2; ++par) {
@@ -885,7 +984,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
 void serfsim_destroy(serfsim_t* h) {
   if (!h) return;
   cudaStreamSynchronize(h->stream);
-  if (getenv("SERFSIM_XTIMING") && !h->mid_ev.empty()) {
+  if (h->sw.xtiming && !h->mid_ev.empty()) {
     double a = 0, b = 0; size_t n = std::min(h->mid_ev.size(), h->tick_ev.size() / 2);
     for (size_t t = 0; t < n; ++t) {
       float x = 0, y = 0;
@@ -915,7 +1014,7 @@ int serfsim_set_topology_csr(serfsim_t* h, const uint64_t* row_ptr, const uint32
   const u64 ne = e1 - e0;
   h->udeg = (h->count && ne % h->count == 0) ? (u32)(ne / h->count) : 0u;
   for (u32 i = 0; i <= h->count && h->udeg; ++i) if (rp[i] != (u64)i * h->udeg) h->udeg = 0;
-  if (const char* e = getenv("SERFSIM_UDEG")) { if (!atoi(e)) h->udeg = 0; }   // A/B: force the general path
+  if (!h->sw.udeg) h->udeg = 0;
   for (size_t i = h->count + 1; i < rp.size(); ++i) rp[i] = (u32)ne;      // padding rows: degree 0
   h->max_tile_edges = 0;
   for (u32 b = 0; b < h->count; b += 256) {
@@ -932,13 +1031,11 @@ int serfsim_set_topology_csr(serfsim_t* h, const uint64_t* row_ptr, const uint32
   // TMA pipeline (single-slot runs): a stage holds the largest tile's CSR span if that is at most 48 KB
   h->stage_col_bytes = 0;
   {
-    int use = 0;   // the direct-load kernel is the default (DESIGN §5); SERFSIM_TMA=1 selects the TMA pipeline
-    if (const char* e = getenv("SERFSIM_TMA")) use = atoi(e);
-    const u32 need = std::max<u32>(h->max_tile_edges * 4u, 16u);
-    if (use && h->R == 1 && need <= 48u * 1024u) h->stage_col_bytes = (need + 127u) & ~127u;
+    const u32 need = std::max<u32>(h->max_tile_edges * 4u, 16u);    // the direct-load kernel is the default (DESIGN §5)
+    if (h->sw.tma && h->R == 1 && need <= 48u * 1024u) h->stage_col_bytes = (need + 127u) & ~127u;
   }
-  h->grid = tick_grid_size(h->count, h->stage_col_bytes ? 3 : h->ctas_per_sm);
-  if (getenv("SERFSIM_VERBOSE")) fprintf(stderr, "serfsim: tick kernel = %s (stage_col_bytes %u, grid %d)\n", h->stage_col_bytes ? "tick_kernel_tma" : "tick_kernel", h->stage_col_bytes, h->grid);
+  h->grid = tick_grid_size(h->count, h->stage_col_bytes ? 3 : h->ctas_per_sm, h->sms, h->sw.gridmul);
+  if (h->sw.verbose) fprintf(stderr, "serfsim: tick kernel = %s (stage_col_bytes %u, grid %d)\n", h->stage_col_bytes ? "tick_kernel_tma" : "tick_kernel", h->stage_col_bytes, h->grid);
   h->has_topo = true;
   h->watch_dirty = true;
   return refresh_watchers(h);
@@ -1007,8 +1104,7 @@ int serfsim_run_until_converged(serfsim_t* h, uint32_t max_ticks, uint32_t* tick
   // runs; in sharded runs it even executes), a synchronisation costs less than two of them.  The leave + fail study (877 ticks, ≈ 70 of
   // them busy) launched 382 ticks per run with chunks of up to 128.
   u32 chunk = 8, chunk_max = 32;
-  if (const char* e = getenv("SERFSIM_CHUNK")) chunk = chunk_max = (u32)std::max(1, atoi(e));
-  const bool host_jump = !getenv("SERFSIM_NO_JUMP");
+  if (h->sw.chunk) chunk = chunk_max = h->sw.chunk;
   const u32 pp = (u32)std::max(0, h->cfg.push_pull_interval_ticks);
   const u32 start = h->tick;
   int rc = 0;
@@ -1037,7 +1133,7 @@ int serfsim_run_until_converged(serfsim_t* h, uint32_t max_ticks, uint32_t* tick
     const u32 n = probe ? 1u : std::min(chunk, max_ticks - (h->tick - start));
     if ((rc = launch_ticks(h, n))) return rc;
     CU(cudaStreamSynchronize(h->stream));
-    if (getenv("SERFSIM_DEBUG_LOOP")) fprintf(stderr, "loop: launched %u ticks -> tick %u, ctl %u %u until %u probe %d chunk %u\n", n, h->tick, h->pin_ctl[0], h->pin_ctl[1], h->pin_ctl[2], (int)probe, chunk);
+    if (h->sw.debug_loop) fprintf(stderr, "loop: launched %u ticks -> tick %u, ctl %u %u until %u probe %d chunk %u\n", n, h->tick, h->pin_ctl[0], h->pin_ctl[1], h->pin_ctl[2], (int)probe, chunk);
     if (*(volatile u32*)h->pin_ctl) {
       const u32 t = ((volatile u32*)h->pin_ctl)[1];
       stop_at(t);
@@ -1049,19 +1145,15 @@ int serfsim_run_until_converged(serfsim_t* h, uint32_t max_ticks, uint32_t* tick
     // produces equal the row before it, and that one must have been judged "not quiescent" by a gate first: a jump is
     // preceded by one single-tick launch (`probe`).
     const u32 until = ((volatile u32*)h->pin_ctl)[2];
-    const bool sleeping = host_jump && until > h->tick && h->tick - start < max_ticks;      // sharded runs: every rank reads the same word
+    const bool sleeping = !h->sw.no_jump && until > h->tick && h->tick - start < max_ticks;      // sharded runs: every rank reads the same word
     // … and the probe tick itself must have been an idle one: with a host operation in it (which may well change nothing) its row is a new
     // one that no gate has judged yet — the next launch is another single tick (found by fuzz scenario 16 once the launch chunks ended
     // on the tick before a no-op operation: the run was reported quiescent at the end of the jump instead of at the operation's tick)
-    bool probe_was_idle = true;
-    if (probe && h->tick > 0) {
-      auto it = std::lower_bound(h->ops.begin(), h->ops.end(), h->tick - 1, [](const HostOp& o, u32 tt) { return o.tick < tt; });
-      probe_was_idle = it == h->ops.end() || it->tick != h->tick - 1;
-    }
+    const bool probe_was_idle = !(probe && h->tick > 0 && ops_at(h, h->tick - 1));
     if (sleeping && probe && probe_was_idle) {
       u32 stop = until;
-      auto nxt = std::lower_bound(h->ops.begin(), h->ops.end(), h->tick, [](const HostOp& o, u32 tt) { return o.tick < tt; });
-      if (nxt != h->ops.end()) stop = std::min(stop, nxt->tick);
+      const u32 nxt = ops_of_tick(h, h->tick).begin;    // the first operation at or after this tick
+      if (nxt < h->ops.size()) stop = std::min(stop, h->ops[nxt].tick);
       const u32 n_skip = std::min(stop > h->tick ? stop - h->tick : 0u, max_ticks - (h->tick - start));
       if (n_skip) {
         if ((rc = ensure_trace(h, h->tick + n_skip + 1))) return rc;
@@ -1071,13 +1163,13 @@ int serfsim_run_until_converged(serfsim_t* h, uint32_t max_ticks, uint32_t* tick
         for (u32 k = 0; k < n_skip; ++k) {
           if (h->tick_timing) {
             const u32 t = h->tick + k;
-            while (h->tick_ev.size() < 2 * ((size_t)t + 1)) { cudaEvent_t e; CU(cudaEventCreate(&e)); h->tick_ev.push_back(e); }
+            if ((rc = grow_events(h->tick_ev, 2 * ((size_t)t + 1)))) return rc;
             CU(cudaEventRecord(h->tick_ev[2 * (size_t)t], h->stream)); CU(cudaEventRecord(h->tick_ev[2 * (size_t)t + 1], h->stream));
           }
           h->launch_log.push_back(k == 0 ? 1u : 0u);
         }
         h->tick += n_skip;
-        if (!getenv("SERFSIM_CHUNK")) chunk = 8;            // the busy stretch after a sleep is short as a rule
+        if (!h->sw.chunk) chunk = 8;            // the busy stretch after a sleep is short as a rule
       }
       probe = false;
     } else {
@@ -1190,13 +1282,8 @@ int serfsim_stats(serfsim_t* h, serfsim_stats_t* o) {
     if (r.pending || r.edge_updates || r.events) o->last_active_tick = i;
   }
   if (!h->rows.empty()) o->pending = h->rows.back().pending;
-  const u32 nout = 2 + 2 * h->R;
-  std::vector<u64> init(nout, 0), out(nout);
-  for (u32 s = 0; s < h->R; ++s) init[2 + 2 * s] = ~0ull;
-  CU(cudaMemcpyAsync(h->d_scratch, init.data(), nout * 8, cudaMemcpyHostToDevice, h->stream));
-  launch_summary(h->d_rec, h->d_qword, h->d_node, h->count, h->stride, h->first, h->R, h->d_subj, h->d_scratch, h->stream);
-  CU(cudaMemcpyAsync(out.data(), h->d_scratch, nout * 8, cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
+  std::vector<u64> out;
+  if ((rc = read_summary(h, out))) return rc;
   o->member_time = out[0]; o->intent_queue = out[1];
   for (u32 s = 0; s < h->R; ++s) if (out[2 + 2 * s] != ~0ull && out[2 + 2 * s] != out[3 + 2 * s]) o->disagree_slots++;
   return 0;
@@ -1268,9 +1355,7 @@ int serfsim_set_user_events(serfsim_t* h, uint32_t n_events, const uint32_t* con
   if (h->cfg.world_size > 1) {
     // every event bit bound for another shard is one window entry: up to fanout · n_events per node and tick on top of the
     // membership entries the windows were sized for.  The windows are exported by serfsim_comm_export, so this must come first.
-    double factor = 1.25;
-    if (const char* e = getenv("SERFSIM_WIN_FACTOR")) factor = atof(e);
-    const double cap = (double)h->win_cap_base + (double)h->shard_size * h->cfg.fanout * n_events * factor / h->cfg.world_size;
+    const double cap = (double)h->win_cap_base + (double)h->shard_size * h->cfg.fanout * n_events * h->sw.win_factor / h->cfg.world_size;
     const u32 want = (u32)std::min(cap, 4.0e9);
     if (want != h->win_cap) {
       if (h->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs call it before serfsim_comm_export / serfsim_comm_connect (it resizes the receive windows)");
@@ -1375,16 +1460,11 @@ int serfsim_user_event_seen(serfsim_t* h, uint32_t event, uint8_t* out) {
 int serfsim_user_event_ltime(serfsim_t* h, uint32_t event, uint64_t* ltime) {
   if (!h || !ltime) return fail(SERFSIM_E_INVAL, "null argument");
   if (event >= h->ue_table.n) return fail(SERFSIM_E_INVAL, "user event index out of range");
-  u32 v = 0;
+  if (h->cfg.world_size > 1 && !h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
+  u32 lt[MAX_UEVENTS];
   CU(cudaStreamSynchronize(h->stream));
-  CU(cudaMemcpy(&v, h->d_ue_ltime + event, 4, cudaMemcpyDeviceToHost));
-  *ltime = v;
-  if (h->cfg.world_size > 1) {                      // the origin's shard stamped it; the others contribute 0 to the sum
-    if (!h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
-    const bool scheduled = (h->ue_injected >> event) & 1u;
-    if (!scheduled || h->ue_origin[event] - h->first >= h->count) *ltime = 0;
-    h->allreduce(h->comm_user, ltime, 1);
-  }
+  if (int rc = ue_cluster_ltimes(h, lt)) return rc;
+  *ltime = lt[event];
   return 0;
 }
 
@@ -1499,34 +1579,14 @@ int serfsim_comm_connect(serfsim_t* h, const void* blobs) {
 #endif
     if ((bs[r].has_snap != 0) != (h->d_snap_rec != nullptr)) return fail(SERFSIM_E_COMM, "push_pull_interval_ticks differs between ranks");
     if (r == h->cfg.rank) { pd[0][r] = h->d_win_data[0]; pd[1][r] = h->d_win_data[1]; pc[r] = h->d_ctrl; psr[r] = h->d_snap_rec; psn[r] = h->d_snap_node; pan[r] = h->d_anomaly; pus[r] = h->d_ue_snap; continue; }
-    void* ptr = nullptr;
     if ((bs[r].has_ue_snap != 0) != (h->d_ue_snap != nullptr)) return fail(SERFSIM_E_COMM, "user events / push-pull configuration differs between ranks");
-    if (bs[r].has_ue_snap) {
-      cudaError_t e = cudaIpcOpenMemHandle(&ptr, bs[r].ue_snap, cudaIpcMemLazyEnablePeerAccess);
-      if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(event snapshot): ") + cudaGetErrorString(e));
-      h->ipc_opened.push_back(ptr); pus[r] = (const uint4*)ptr;
-    }
-    {
-      cudaError_t e = cudaIpcOpenMemHandle(&ptr, bs[r].anomaly, cudaIpcMemLazyEnablePeerAccess);
-      if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(flags): ") + cudaGetErrorString(e));
-      h->ipc_opened.push_back(ptr); pan[r] = (u8*)ptr;
-    }
-    if (bs[r].has_snap) {
-      cudaError_t e = cudaIpcOpenMemHandle(&ptr, bs[r].snap_rec, cudaIpcMemLazyEnablePeerAccess);
-      if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(snapshot): ") + cudaGetErrorString(e));
-      h->ipc_opened.push_back(ptr); psr[r] = (const uint4*)ptr;
-      e = cudaIpcOpenMemHandle(&ptr, bs[r].snap_node, cudaIpcMemLazyEnablePeerAccess);
-      if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(snapshot): ") + cudaGetErrorString(e));
-      h->ipc_opened.push_back(ptr); psn[r] = (const u64*)ptr;
-    }
-    for (int par = 0; par < 2; ++par) {
-      cudaError_t e = cudaIpcOpenMemHandle(&ptr, bs[r].data[par], cudaIpcMemLazyEnablePeerAccess);
-      if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(window): ") + cudaGetErrorString(e));
-      h->ipc_opened.push_back(ptr); pd[par][r] = (u64*)ptr;
-    }
-    cudaError_t e = cudaIpcOpenMemHandle(&ptr, bs[r].ctrl, cudaIpcMemLazyEnablePeerAccess);
-    if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(ctrl): ") + cudaGetErrorString(e));
-    h->ipc_opened.push_back(ptr); pc[r] = (u32*)ptr;
+    int rc = bs[r].has_ue_snap ? ipc_open(h, bs[r].ue_snap, "event snapshot", &pus[r]) : 0;
+    if (!rc) rc = ipc_open(h, bs[r].anomaly, "flags", &pan[r]);
+    if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_rec, "snapshot", &psr[r]);
+    if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_node, "snapshot", &psn[r]);
+    for (int par = 0; par < 2 && !rc; ++par) rc = ipc_open(h, bs[r].data[par], "window", &pd[par][r]);
+    if (!rc) rc = ipc_open(h, bs[r].ctrl, "ctrl", &pc[r]);
+    if (rc) return rc;
   }
   for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), sizeof(u64*) * 8, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), sizeof(u32*) * 8, cudaMemcpyHostToDevice));

@@ -1620,18 +1620,9 @@ __global__ void __launch_bounds__(BLOCK) summary_kernel(const uint4* rec, const 
 int tick_ctas_per_sm_r1() { return SFS_MB_R1; }
 int tick_ctas_per_sm_r1s() { return SFS_MB_R1S; }
 int tick_ctas_per_sm_rn() { return SFS_MB_RN; }
-int tick_grid_size(u32 n_local, int ctas_per_sm) {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-  }
+int tick_grid_size(u32 n_local, int ctas_per_sm, int sms, int gridmul) {
   const u32 tiles = (n_local + BLOCK - 1) / BLOCK;
-  static int mul = 0;
-  if (!mul) { const char* e = getenv("SERFSIM_GRIDMUL"); mul = e ? atoi(e) : 2; if (mul < 1) mul = 2; }
-  u32 grid = (u32)sms * (u32)ctas_per_sm * (u32)mul;    // persistent: SM count × resident CTAs × 2 (two waves for balance)
+  u32 grid = (u32)sms * (u32)ctas_per_sm * (u32)gridmul;    // persistent: SM count × resident CTAs × 2 (two waves for balance)
   if (tiles < grid) grid = tiles ? tiles : 1;
   while ((tiles + grid - 1) / grid > MAX_TILES_PER_CTA) grid += (u32)sms * (u32)ctas_per_sm;
   return (int)grid;
@@ -1639,14 +1630,12 @@ int tick_grid_size(u32 n_local, int ctas_per_sm) {
 
 #ifndef SERFSIM_EMU
 template <bool TRACE, int FMAX, bool SHARDED>
-static void launch_tick_tma(const TickParams& p, int grid, cudaStream_t st) {
+static void launch_tick_tma(const TickParams& p, int grid, bool barsync, cudaStream_t st) {
   const size_t smem = 2 * (size_t)(ST_COL + p.stage_col_bytes);
   static bool configured = false;
-  static int barsync = 0;
   if (!configured) {
     cudaFuncSetAttribute(tick_kernel_tma<TRACE, FMAX, SHARDED, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(tick_kernel_tma<TRACE, FMAX, SHARDED, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (const char* e = getenv("SERFSIM_TMA_SYNC")) barsync = atoi(e);
     configured = true;
   }
   if (barsync) SFS_LAUNCH(grid, BLOCK, smem, st, tick_kernel_tma<TRACE, FMAX, SHARDED, true>)(p);
@@ -1655,24 +1644,22 @@ static void launch_tick_tma(const TickParams& p, int grid, cudaStream_t st) {
 #endif
 
 template <bool TRACE, int FMAX>
-static void launch_tick_v(const TickParams& p, int grid, cudaStream_t st) {
+static void launch_tick_v(const TickParams& p, int grid, int ctas_per_sm, bool tma_sync, cudaStream_t st) {
   const bool sharded = p.world > 1, r1 = p.R == 1;
 #ifndef SERFSIM_EMU
   if (r1 && p.stage_col_bytes && !sharded) { // single-slot, single-GPU run whose tiles fit a shared-memory stage: TMA pipeline
-    launch_tick_tma<TRACE, FMAX, false>(p, grid, st);
+    launch_tick_tma<TRACE, FMAX, false>(p, grid, tma_sync, st);
     return;
   }
 #endif
-  static int mb5 = -1;
-  if (mb5 < 0) { const char* e = getenv("SERFSIM_MINB"); mb5 = (e && atoi(e) == 5) ? 1 : 0; }
   if (sharded) { if (r1) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, true, true, SFS_MB_R1S>)(p); else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, true, false, SFS_MB_RN>)(p); }
-  else if (r1) { if (mb5) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, false, true, 5>)(p); else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, false, true, SFS_MB_R1>)(p); }
+  else if (r1) { if (ctas_per_sm == 5) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, false, true, 5>)(p); else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, false, true, SFS_MB_R1>)(p); }
   else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<TRACE, FMAX, false, false, SFS_MB_RN>)(p);
 }
-void launch_tick(const TickParams& p, bool trace, int grid, cudaStream_t st) {
+void launch_tick(const TickParams& p, bool trace, int grid, int ctas_per_sm, bool tma_sync, cudaStream_t st) {
   const bool small = p.fanout <= 4;          // the common fan-outs (3, 4) get the 4-wide target array
-  if (trace) { if (small) launch_tick_v<true, 4>(p, grid, st); else launch_tick_v<true, 8>(p, grid, st); }
-  else { if (small) launch_tick_v<false, 4>(p, grid, st); else launch_tick_v<false, 8>(p, grid, st); }
+  if (trace) { if (small) launch_tick_v<true, 4>(p, grid, ctas_per_sm, tma_sync, st); else launch_tick_v<true, 8>(p, grid, ctas_per_sm, tma_sync, st); }
+  else { if (small) launch_tick_v<false, 4>(p, grid, ctas_per_sm, tma_sync, st); else launch_tick_v<false, 8>(p, grid, ctas_per_sm, tma_sync, st); }
 }
 // One pass of a tick of an unsharded multi-slot run (SV_PASS): the single-slot kernel on the view the parameter block starts at.
 void launch_tick_pass(const TickParams& p, int grid, cudaStream_t st) {

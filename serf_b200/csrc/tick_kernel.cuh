@@ -208,7 +208,9 @@ struct DrainParams {
   u32 tick, sleep_on;
 };
 
-void launch_tick(const TickParams& p, bool trace, int grid, cudaStream_t st);
+// ctas_per_sm: the resident CTAs per SM the grid was sized for (5 picks the 5-CTA instance of the unsharded single-slot kernel);
+// tma_sync: the TMA pipeline's barrier-synchronised form (SERFSIM_TMA_SYNC)
+void launch_tick(const TickParams& p, bool trace, int grid, int ctas_per_sm, bool tma_sync, cudaStream_t st);
 void launch_tick_single_view(const TickParams& p, int grid, cudaStream_t st);
 void launch_tick_pass(const TickParams& p, int grid, cudaStream_t st);
 void launch_fill_idle_rows(u64* rows, u64* grow_rows, u32 n, const u32* sched, bool trace, cudaStream_t st);
@@ -221,7 +223,7 @@ void launch_extract(const uint4* rec, const u64* node_state, u32 n_local, u32 st
 void launch_compose_records(const uint4* rec, const u32* qword, u32 n_local, u32 stride, u32 slot, uint4* out, cudaStream_t st);
 void launch_state_hash(const uint4* rec, const u32* qword, const u64* node_state, u32 n_local, u32 stride, u32 first, u32 n_global, u32 R, u64* out, cudaStream_t st);
 void launch_summary(const uint4* rec, const u32* qword, const u64* node_state, u32 n_local, u32 stride, u32 first, u32 R, const u32* subj_dev, u64* out /*[2 + 2*R + 2]*/, cudaStream_t st);
-int tick_grid_size(u32 n_local, int ctas_per_sm);
+int tick_grid_size(u32 n_local, int ctas_per_sm, int sms, int gridmul);
 int tick_ctas_per_sm_r1();
 int tick_ctas_per_sm_r1s();
 int tick_ctas_per_sm_rn();

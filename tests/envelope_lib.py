@@ -9,9 +9,12 @@ test infrastructure only.
   graphs.
 - kernel_lines: the kernel and grid the library prints for each topology under SERFSIM_VERBOSE.
 - product_run: a run's parity outputs (parity_lib.outputs) with the product-only getters beside them.
-- run_isolated: product_run in a fresh process.  SERFSIM_GRIDMUL, SERFSIM_MINB and SERFSIM_TMA_SYNC are read once per process (the
-  first launch fixes them), so a variant selected by them only runs in a process of its own.
+- run_jobs / grid_for: product runs / a handle's kernel and grid under a set of run-time switches, in this process (every handle reads
+  the switches when it is created).
+- run_isolated: product_run in a fresh process, for the host build's lane and CTA schedule (SERFSIM_EMU_SCHED), which the host build
+  reads once per process.
 """
+import contextlib
 import os
 import pickle
 import re
@@ -20,6 +23,7 @@ import sys
 import tempfile
 
 import numpy as np
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
@@ -191,25 +195,57 @@ def product_run(sim, sc):
     return dict(out=out, view_kinds=sim.tick_view_kinds(), launches=sim.last_step_device_ms()[1])
 
 
+@contextlib.contextmanager
+def switches(env=None):
+    """The run-time switches `env` and SERFSIM_VERBOSE=1 for the handles created inside.  On the host build of the kernels
+    (SERFSIM_GPU_TESTS_ON_EMU=1) the device has 4 SMs unless SERFSIM_EMU_SMS says otherwise: 12 CTAs of the single-slot kernel at
+    SERFSIM_GRIDMUL=1."""
+    with pytest.MonkeyPatch.context() as mp:
+        for k, v in (env or {}).items():
+            mp.setenv(k, v)
+        mp.setenv("SERFSIM_VERBOSE", "1")
+        if ON_EMU and not os.environ.get("SERFSIM_EMU_SMS"):
+            mp.setenv("SERFSIM_EMU_SMS", "4")
+        yield
+
+
+def run_jobs(jobs, capfd, env=None):
+    """Run jobs — dict(sc=Scenario, trace=0/1, cfg={...}) — through the product library (the host build under
+    SERFSIM_GPU_TESTS_ON_EMU=1) under the switches `env`.  Returns one product_run dict per job, with "kernel": (kernel name, grid)
+    of the job's topology (kernel_lines, read from the captured stderr)."""
+    from serf_b200 import GossipSim
+    res = []
+    with switches(env):
+        for job in jobs:
+            capfd.readouterr()
+            sim = job["sc"].build(GossipSim, trace=job["trace"], **job.get("cfg", {}))
+            r = product_run(sim, job["sc"])
+            sim.close()
+            lines = kernel_lines(capfd.readouterr().err)
+            assert len(lines) == 1, lines                  # every job sets one topology
+            res.append(dict(r, kernel=lines[0]))
+    return res
+
+
+def grid_for(factory, n, capfd, env=None):
+    """(kernel name, grid) an n-node single-slot handle made by `factory` picks under the switches `env`."""
+    with switches(env):
+        capfd.readouterr()
+        g = factory(n, 1)
+        g.set_topology(np.arange(n + 1, dtype=np.uint64), ((np.arange(n) + 1) % n).astype(np.uint32))
+        g.close()
+        (line,) = kernel_lines(capfd.readouterr().err)
+    return line
+
+
 def _child(job_path, out_path):
-    from serf_b200 import GossipSim, sim as _sim
-    if ON_EMU:
-        sys.path.insert(0, os.path.join(ROOT, "tests"))
-        import emu_lib
-        _sim._LIB = emu_lib.lib()
+    from emu_lib import emu_sim
     with open(job_path, "rb") as f:
         jobs = pickle.load(f)
     res = []
     for job in jobs:
-        if job.get("probe"):                              # the grid of a handle of job["probe"] nodes: nothing is run
-            n = job["probe"]
-            g = GossipSim(n, 1)
-            g.set_topology(np.arange(n + 1, dtype=np.uint64), ((np.arange(n) + 1) % n).astype(np.uint32))
-            g.close()
-            res.append(None)
-            continue
-        sc, trace = job["sc"], job["trace"]
-        g = sc.build(GossipSim, trace=trace, **job.get("cfg", {}))
+        sc = job["sc"]
+        g = sc.build(emu_sim, trace=job["trace"], **job.get("cfg", {}))
         res.append(product_run(g, sc))
         g.close()
     with open(out_path, "wb") as f:
@@ -217,14 +253,11 @@ def _child(job_path, out_path):
 
 
 def run_isolated(jobs, env=None, timeout=1200):
-    """Run jobs — dict(sc=Scenario, trace=0/1, cfg={...}) or dict(probe=n) — through the product library (the host build under
-    SERFSIM_GPU_TESTS_ON_EMU=1) in a new Python process with `env` added to this one's and SERFSIM_VERBOSE=1.
-    Returns one product_run dict per job, with "kernel": (kernel name, grid) of the job's topology (kernel_lines)."""
+    """Run jobs — dict(sc=Scenario, trace=0/1, cfg={...}) — through the host build of the kernels in a new Python process with `env`
+    added to this one's.  The host build reads its lane and CTA schedule (SERFSIM_EMU_SCHED, tests/emu/emu_engine.cpp) once per
+    process, so a run under another schedule needs a process of its own.  Returns one product_run dict per job."""
     e = dict(os.environ)
     e.update(env or {})
-    e["SERFSIM_VERBOSE"] = "1"
-    if ON_EMU:
-        e.setdefault("SERFSIM_EMU_SMS", "4")            # the host build's grid: 12 CTAs of the single-slot kernel at SERFSIM_GRIDMUL=1
     with tempfile.TemporaryDirectory(prefix="serfsim_envelope_") as d:
         jp, op = os.path.join(d, "jobs.pkl"), os.path.join(d, "out.pkl")
         with open(jp, "wb") as f:
@@ -232,15 +265,7 @@ def run_isolated(jobs, env=None, timeout=1200):
         p = subprocess.run([sys.executable, os.path.abspath(__file__), jp, op], env=e, cwd=ROOT, capture_output=True, text=True, timeout=timeout)
         assert p.returncode == 0, f"child run failed ({p.returncode}):\n{p.stderr[-4000:]}"
         with open(op, "rb") as f:
-            res = pickle.load(f)
-    lines = kernel_lines(p.stderr)                        # one per job: every job sets one topology
-    assert len(lines) == len(jobs), p.stderr[-4000:]
-    return [dict(r or {}, kernel=k) for r, k in zip(res, lines)]
-
-
-def grid_for(n, env=None):
-    """(kernel name, grid) the library picks for an n-node single-slot handle under `env`."""
-    return run_isolated([dict(probe=n)], env)[0]["kernel"]
+            return pickle.load(f)
 
 
 if __name__ == "__main__":

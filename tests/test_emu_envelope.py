@@ -23,6 +23,15 @@ def probes():
 
 
 # ---- irregular CSR -------------------------------------------------------------------------------------------
+def test_each_handle_reads_its_own_switches(capfd):
+    """The run-time switches are read when a handle is created: in one process, a handle under SERFSIM_GRIDMUL=1 gets one wave of
+    CTAs and the next one, without it, two."""
+    n = 64 * E.TILE
+    one = E.grid_for(emu_sim, n, capfd, {"SERFSIM_GRIDMUL": "1", "SERFSIM_EMU_SMS": "4"})
+    two = E.grid_for(emu_sim, n, capfd, {"SERFSIM_EMU_SMS": "4"})
+    assert one[1] == 4 * 3 and two == (one[0], 2 * one[1]), (one, two)
+
+
 def test_irregular_graph_shape():
     rp, col = E.irregular_graph(20_000, 1, self_loops=0.05, duplicates=0.05)
     deg = np.diff(rp.astype(np.int64))

@@ -48,11 +48,10 @@ def test_long_run_grows_the_trace_buffer():
     P.assert_same(P.outputs(g, sc, tg), P.outputs(o, sc, to), with_hash=True)
 
 
-def test_speculative_pipeline_gives_the_same_result(monkeypatch):
+def test_launch_chunks_1_4_16_give_the_same_result(monkeypatch):
     sc = scenarios.random_graph_leave(3000, 12, 4, seed=3)
     o = sc.build(oracle_sim, trace=1)
     ref = P.outputs(o, sc, o.run_until_converged(sc.max_ticks))
-    monkeypatch.setenv("SERFSIM_SPECULATE", "1")
     for chunk in ("1", "4", "16"):
         monkeypatch.setenv("SERFSIM_CHUNK", chunk)
         g = sc.build(emu_sim, trace=0)

@@ -75,7 +75,7 @@ def test_fuzz_prune(seed):
     P.run_against_oracle(emu_sim, scenarios.fuzz_prune(seed))
 
 
-def test_sleeping_views_timer_wheel_and_idle_ticks():
+def test_sleeping_views_timer_wheel_and_idle_ticks(monkeypatch):
     """A crash with the memberlist LAN timers: the suspicion timers run for ~100 ticks in which nothing else happens.  Views that
     only wait for their timer sleep (SFS_PROBE 5 counts the views a visited node left asleep), their tiles are woken by the
     timer wheel (probe 4) and the ticks in which nothing can happen are skipped (probe 3) — with every trace row, `pending`
@@ -89,16 +89,14 @@ def test_sleeping_views_timer_wheel_and_idle_ticks():
     to = o.run_until_converged(sc.max_ticks)
     ref = P.outputs(o, sc, to)
     assert to[0] > 60
-    import os
     for trace, chunk in ((0, None), (1, None), (0, "4"), (1, "5")):
         L.emu_probe_reset()
-        f = sc.build(emu_sim, trace=trace)
         if chunk:
-            os.environ["SERFSIM_CHUNK"] = chunk            # small launch chunks: the host learns early that the cluster sleeps
-        try:
-            got = P.outputs(f, sc, f.run_until_converged(sc.max_ticks))
-        finally:
-            os.environ.pop("SERFSIM_CHUNK", None)
+            monkeypatch.setenv("SERFSIM_CHUNK", chunk)     # small launch chunks: the host learns early that the cluster sleeps
+        else:
+            monkeypatch.delenv("SERFSIM_CHUNK", raising=False)
+        f = sc.build(emu_sim, trace=trace)
+        got = P.outputs(f, sc, f.run_until_converged(sc.max_ticks))
         # skipped on the device (launched before the host learnt that the cluster sleeps, probe 3) or not launched at all (probe 17)
         assert L.emu_probe(3) + L.emu_probe(17) > 20 and L.emu_probe(4) > 0, (L.emu_probe(3), L.emu_probe(17), L.emu_probe(4))
         if chunk:

@@ -31,9 +31,9 @@ def device_sim(n, slots=1, **kw):
     return GossipSim(n, slots, **kw)
 
 
-def check(jobs):
-    """Run the jobs through the library in a fresh process and compare each with the oracle (trace = 1)."""
-    res = E.run_isolated(jobs)
+def check(jobs, capfd):
+    """Run the jobs through the library and compare each with the oracle (trace = 1)."""
+    res = E.run_jobs(jobs, capfd)
     oracles = {}
     for job, got in zip(jobs, res):
         sc = job["sc"]
@@ -45,21 +45,21 @@ def check(jobs):
     return res
 
 
-def test_config_fuzz_small():
+def test_config_fuzz_small(capfd):
     scs = [CL.config_fuzz(s) for s in range(40)]
-    check([dict(sc=sc, trace=t) for sc in scs for t in (1, 0)])
+    check([dict(sc=sc, trace=t) for sc in scs for t in (1, 0)], capfd)
 
 
 LARGE = (9_999, 10_000, 10_001, 99_999, 100_000, 100_001)
 
 
 @pytest.mark.parametrize("n", LARGE)
-def test_config_fuzz_at_a_power_of_ten(n):
+def test_config_fuzz_at_a_power_of_ten(n, capfd):
     """Drawn configs at 10^4 / 10^5 ± 1 nodes: the retransmit limit gains a digit and the node scale is exact at 10^k."""
     n = size(n, n // 100 + n % 10)
     sc = CL.config_fuzz(9_000 + n, n=n)
     sc.max_ticks = 200
-    check([dict(sc=sc, trace=1), dict(sc=sc, trace=0)])
+    check([dict(sc=sc, trace=1), dict(sc=sc, trace=0)], capfd)
 
 
 def test_lifeguard_k7_full_confirmer_sets():
@@ -102,7 +102,7 @@ def _budget_check(stats, limit, n):
 
 
 @pytest.mark.parametrize("mult,n", [(63, 5_000), (63, 9_999)])
-def test_transmit_budget_252(mult, n):
+def test_transmit_budget_252(mult, n, capfd):
     """retransmit_mult 63 at 1000–9999 nodes: a limit of 252 through the single-slot kernels (a leave study and a crash study)."""
     limit = CL.expected_retransmit_limit(mult, n)
     assert limit == 252
@@ -111,7 +111,7 @@ def test_transmit_budget_252(mult, n):
     crash = E.crash_study(n, topo, fanout=4, seed=3, short_timers=True, max_ticks=600)
     for sc in (leave, crash):
         sc.cfg["retransmit_mult"] = mult
-    res = check([dict(sc=sc, trace=t) for sc in (leave, crash) for t in (1, 0)])
+    res = check([dict(sc=sc, trace=t) for sc in (leave, crash) for t in (1, 0)], capfd)
     _budget_check(res[0]["out"]["stats"], limit, n)
 
 

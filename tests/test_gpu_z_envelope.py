@@ -10,8 +10,8 @@ and in production mode:
 - the scheduler switches SERFSIM_NO_SKIP / SERFSIM_NO_JUMP;
 - fan-out 6–8 with 9–16 slots, run as per-view passes.
 
-SERFSIM_GRIDMUL, SERFSIM_MINB and SERFSIM_TMA_SYNC are read once per process, so every device run here happens in a process of
-its own (envelope_lib.run_isolated), which also reports the kernel and grid SERFSIM_VERBOSE printed for it."""
+Every run reads its switches when its handle is created (envelope_lib.run_jobs), and reports the kernel and grid SERFSIM_VERBOSE
+printed for it."""
 import functools
 
 import pytest
@@ -19,6 +19,7 @@ import pytest
 import envelope_lib as E
 import parity_lib as P
 from oracle_lib import oracle_sim, oracle_sim_threaded
+from serf_b200 import GossipSim
 from serf_b200.sim import random_regular_graph
 from test_gpu_z_multislot_paths import MODES
 
@@ -46,9 +47,9 @@ def oracle(sc, cfg=None):
     return _ORACLES[key][1]
 
 
-def check(jobs, env, expect_kernel=None):
-    """Run the jobs in a fresh process under env and compare each with the oracle; returns the outputs."""
-    res = E.run_isolated(jobs, env)
+def check(jobs, env, capfd, expect_kernel=None):
+    """Run the jobs under the switches env and compare each with the oracle; returns the outputs."""
+    res = E.run_jobs(jobs, capfd, env)
     for job, got in zip(jobs, res):
         sc = job["sc"]
         what = f"{sc.name} trace={job['trace']} {env}"
@@ -75,29 +76,29 @@ def irregular_scenarios():
 
 
 @pytest.mark.parametrize("kernel", list(KERNELS))
-def test_irregular_csr(kernel):
+def test_irregular_csr(kernel, capfd):
     env, name = KERNELS[kernel]
     studies, fz = irregular_scenarios()
-    check(both(*studies) + both(*fz), env, name)
+    check(both(*studies) + both(*fz), env, capfd, name)
 
 
-def test_uniform_graph_forced_through_general_path():
+def test_uniform_graph_forced_through_general_path(capfd):
     n = size(100_000, 8000)
     sc = E.crash_study(n, random_regular_graph(n, 16, 9), fanout=4, short_timers=True)
-    a = check(both(sc), {})
-    b = check(both(sc), {"SERFSIM_UDEG": "0"})
+    a = check(both(sc), {}, capfd)
+    b = check(both(sc), {"SERFSIM_UDEG": "0"}, capfd)
     for x, y in zip(a, b):
         P.assert_same(y["out"], x["out"], with_hash=True, what="SERFSIM_UDEG=0")
 
 
 # ---- TMA stage boundary ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("over", [0, 4], ids=["at_48k", "one_edge_over"])
-def test_tma_stage_boundary(over):
+def test_tma_stage_boundary(over, capfd):
     n = size(60_000, 4000)
     topo = E.tma_span_graph(n, E.TMA_STAGE_BYTES + over)
     assert E.max_tile_span_bytes(topo[0]) == E.TMA_STAGE_BYTES + (16 if over else 0)
     scs = (E.leave_study(n, topo, fanout=4), E.crash_study(n, topo, fanout=3, short_timers=True))
-    check(both(*scs), {"SERFSIM_TMA": "1"}, DIRECT if over else TMA)
+    check(both(*scs), {"SERFSIM_TMA": "1"}, capfd, DIRECT if over else TMA)
 
 
 # ---- several tiles per CTA --------------------------------------------------------------------------------------------
@@ -108,10 +109,9 @@ MULTI = {"direct": ({"SERFSIM_GRIDMUL": "1"}, DIRECT, TILES_PER_CTA), "tma": ({"
 
 
 @functools.lru_cache(None)
-def multi_tile_scenarios():
-    """n from the direct kernel's printed grid G: T = 8·G + 1 tiles gives every busy CTA ⌈T / G⌉ = 9 tiles, leaves the CTAs
+def multi_tile_scenarios(g):
+    """n from the direct kernel's printed grid g: T = 8·g + 1 tiles gives every busy CTA ⌈T / g⌉ = 9 tiles, leaves the CTAs
     past ⌈T / 9⌉ empty and the last busy one a single tile; the last tile holds 77 nodes."""
-    _, g = E.grid_for(1 << 20, {"SERFSIM_GRIDMUL": "1"})
     tiles = (TILES_PER_CTA - 1) * g + 1
     n = (tiles - 1) * E.TILE + 77
     topo = random_regular_graph(n, 16, 7)
@@ -119,11 +119,12 @@ def multi_tile_scenarios():
 
 
 @pytest.mark.parametrize("variant", list(MULTI))
-def test_several_tiles_per_cta(variant):
+def test_several_tiles_per_cta(variant, capfd):
     env, name, min_tiles = MULTI[variant]
-    n, g0, (leave, crash_lan, crash_short) = multi_tile_scenarios()
+    _, g = E.grid_for(GossipSim, 1 << 20, capfd, {"SERFSIM_GRIDMUL": "1"})
+    n, g0, (leave, crash_lan, crash_short) = multi_tile_scenarios(g)
     jobs = both(leave) + [dict(sc=crash_lan, trace=0), dict(sc=crash_short, trace=0)]   # timer-wheel studies: production mode
-    res = check(jobs, env, name)
+    res = check(jobs, env, capfd, name)
     grid = res[0]["kernel"][1]
     per = E.tiles_per_cta(n, grid)
     print(f"{variant}: n {n}, grid {grid}, {per} tiles per CTA, {E.busy_ctas(n, grid)} CTAs with tiles")
@@ -141,18 +142,23 @@ def switch_scenarios():
     return [crash, storm], [E.envelope_fuzz(s) for s in range(8)]
 
 
-@functools.lru_cache(None)
-def default_switch_runs():
-    studies, fz = switch_scenarios()
-    return check(both(*studies) + [dict(sc=sc, trace=0) for sc in fz], {})
+_DEFAULT_SWITCH_RUNS = []
+
+
+def default_switch_runs(capfd):
+    """The scheduler-switch scenarios without a switch, run once for every test that compares with them."""
+    if not _DEFAULT_SWITCH_RUNS:
+        studies, fz = switch_scenarios()
+        _DEFAULT_SWITCH_RUNS.extend(check(both(*studies) + [dict(sc=sc, trace=0) for sc in fz], {}, capfd))
+    return _DEFAULT_SWITCH_RUNS
 
 
 @pytest.mark.parametrize("env", [{"SERFSIM_NO_SKIP": "1"}, {"SERFSIM_NO_JUMP": "1"}, {"SERFSIM_NO_SKIP": "1", "SERFSIM_NO_JUMP": "1"}],
                          ids=["no_skip", "no_jump", "both"])
-def test_scheduler_switches(env):
+def test_scheduler_switches(env, capfd):
     studies, fz = switch_scenarios()
-    res = check(both(*studies) + [dict(sc=sc, trace=0) for sc in fz], env)
-    for got, base in zip(res, default_switch_runs()):
+    res = check(both(*studies) + [dict(sc=sc, trace=0) for sc in fz], env, capfd)
+    for got, base in zip(res, default_switch_runs(capfd)):
         P.assert_same(got["out"], base["out"], with_hash=True, what=str(env))
 
 
@@ -174,22 +180,22 @@ def wide_storm():
 
 
 @pytest.mark.parametrize("mode", MODES, ids=lambda m: ",".join(f"{k[8:]}={v}" for k, v in m.items()))
-def test_fanout8_slots12_storm(mode):
+def test_fanout8_slots12_storm(mode, capfd):
     sc = wide_storm()
-    check(both(sc), mode)
+    check(both(sc), mode, capfd)
 
 
-def test_wide_fuzz():
+def test_wide_fuzz(capfd):
     scs = [E.envelope_fuzz(s) for s in wide_fuzz_seeds(16)]
     assert {sc.cfg["fanout"] for sc in scs} == {6, 7, 8} and max(sc.slots for sc in scs) >= 15
     for mode in (MODES[0], MODES[1]):
-        check([dict(sc=sc, trace=0) for sc in scs], mode)
+        check([dict(sc=sc, trace=0) for sc in scs], mode, capfd)
 
 
-def test_per_view_passes_ran():
+def test_per_view_passes_ran(capfd):
     """Production run of the storm: every tick that runs as passes launches R kernels instead of one, so SERFSIM_SV=1 launches
     more kernels than SERFSIM_SV=0 — at least R − 1 = 11 more per tick for the ticks without a host operation."""
     sc = wide_storm()
-    off = check([dict(sc=sc, trace=0)], {"SERFSIM_SV": "0"})[0]
-    on = check([dict(sc=sc, trace=0)], {"SERFSIM_SV": "1"})[0]
+    off = check([dict(sc=sc, trace=0)], {"SERFSIM_SV": "0"}, capfd)[0]
+    on = check([dict(sc=sc, trace=0)], {"SERFSIM_SV": "1"}, capfd)[0]
     assert on["launches"] >= off["launches"] + (sc.slots - 1) * 5, (on["launches"], off["launches"])

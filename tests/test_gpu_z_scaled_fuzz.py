@@ -7,7 +7,7 @@ Only a multi-CTA launch on feature-rich traffic can show a race or an ordering m
 marks of sparse ticks, tile_due / node_due, the last-CTA ticket and sleep verdict, the carry words between passes, the per-view kind
 counters or the scheduler's jump rule.  A subset of the seeds runs again under every run-time switch (SERFSIM_SV 0 / 2,
 SERFSIM_COMPACT=0, SERFSIM_AHEAD 0 / 2, SERFSIM_DEDUP=0, SERFSIM_NO_SKIP, SERFSIM_NO_JUMP, SERFSIM_CHUNK 3–7, SERFSIM_TMA=1 on the
-single-slot seeds) and in fresh processes under SERFSIM_GRIDMUL=1 (several tiles per CTA).  The paths reached are derived from the
+single-slot seeds) and under SERFSIM_GRIDMUL=1 (several tiles per CTA).  The paths reached are derived from the
 product's getters (scaled_fuzz_lib.reach) and asserted: a parity test that never reached them would prove little."""
 import functools
 
@@ -119,12 +119,12 @@ def test_tma_on_single_slot_seeds(monkeypatch):
             P.assert_same(run(sc, trace)["out"], ref, with_hash=bool(trace), what=f"{sc.name} TMA trace={trace}")
 
 
-def test_several_tiles_per_cta():
-    """SERFSIM_GRIDMUL=1 (read once per process): one wave of CTAs instead of two.  The multi-slot kernel runs one CTA per SM, so above
+def test_several_tiles_per_cta(capfd):
+    """SERFSIM_GRIDMUL=1: one wave of CTAs instead of two.  The multi-slot kernel runs one CTA per SM, so above
     132 · 256 nodes each of its CTAs owns several tiles — the multi-tile compaction groups of host-operation and reaper ticks."""
     seeds = [s for s in SEEDS if scenario(s).slots > 1 and scenario(s).n > size(40_000, 0)][:3]
     assert len(seeds) == 3
-    res = E.run_isolated([dict(sc=oracle(s)[0], trace=t) for s in seeds for t in (1, 0)], {"SERFSIM_GRIDMUL": "1"})
+    res = E.run_jobs([dict(sc=oracle(s)[0], trace=t) for s in seeds for t in (1, 0)], capfd, {"SERFSIM_GRIDMUL": "1"})
     for i, got in enumerate(res):
         sc, ref = oracle(seeds[i // 2])
         P.assert_same(got["out"], ref, with_hash=i % 2 == 0, what=f"{sc.name} GRIDMUL=1")
