@@ -22,15 +22,14 @@ __global__ void __launch_bounds__(128) byz_kernel(const __grid_constant__ ByzPar
     const u32 u = p.ids[i];
     const u32 ul = u - p.first;
     const u64 ns = p.node_state[ul];
-    if (ns & NS_UP) {                                          // up after this tick's operations
+    if (nw_up(ns)) {                                           // up after this tick's operations
       const u32 row0 = p.row_ptr[ul], deg = p.row_ptr[ul + 1] - row0;
       u32 tg[MAX_FANOUT];
       const u32 nt = ue_pick_targets(p.tick, u, row0, deg, p.fanout, p.seed_lo, p.seed_hi, p.col, tg);
       bool flag = false;
       for (u32 s = 0; s < p.R; ++s) {
-        const size_t iu = (size_t)s * p.stride + ul;
         Rec r;
-        unpack(p.rec[2 * iu], p.rec[2 * iu + 1], r);
+        unpack(load_rec(p.rec, (size_t)s * p.stride + ul), r);
         const ByzEntries e = byz_entries(r, p.delta);
         if (!e.any) continue;
         u32* const planeS = p.inbox_wr + (size_t)(e.serf_kind * p.R + s) * p.stride;
@@ -41,27 +40,19 @@ __global__ void __launch_bounds__(128) byz_kernel(const __grid_constant__ ByzPar
           n_msgs += 2; n_edges += 1;
           if (p.world > 1 && dl >= p.n_local) {                // the peer lives in another shard: triple into its window
             const u32 shard = tg[k] / p.shard_size, dloc = (tg[k] - shard * p.shard_size) | BYZ_FLAG;
-            const u32 g = atomicAdd(p.send_count + shard, 3u);
-            if (g + 3 <= p.win_cap) {
-              u64* w = p.win_data[shard] + (size_t)p.rank * p.win_cap + g;
-              w[0] = ((u64)serf_val1 << 32) | ((u64)s << 28) | ((u64)e.serf_kind << 26) | dloc;
-              w[1] = ((u64)(e.ml_key + 1u) << 32) | ((u64)s << 28) | ((u64)KIND_ML << 26) | dloc;
-              w[2] = ((u64)(u + 1u) << 32) | ((u64)BYZ_ANNOT_SLOT << 28) | (3ull << 26) | dloc;
-            } else {
-              *p.overflow = 2;
-            }
+            win_append<3>(p, shard, {win_entry(serf_val1, s, e.serf_kind, dloc), win_entry(e.ml_key + 1u, s, KIND_ML, dloc),
+                                     win_entry(u + 1u, BYZ_ANNOT_SLOT, KIND_EXTRA, dloc)});
             wrote_remote = true;
             continue;                                          // kinds / tile flags / verdict are the receiving shard's business
           }
           atomicMax(planeS + dl, serf_val1);
           atomicMax(planeM + dl, e.ml_key + 1u);
-          p.hot_wr[dl >> 8] = 1;                               // TILE_SHIFT = 8: the destination tile must run next tick
+          p.hot_wr[dl >> TILE_SHIFT] = 1;                      // the destination tile must run next tick
           if (e.serf_kind == KIND_LEAVE) ++kL; else ++kJ;
           ++kM;
-          if (p.node_state[dl] & NS_UP) {                      // the receiver is up when the packet arrives
-            const size_t iv = (size_t)s * p.stride + dl;
+          if (nw_up(p.node_state[dl])) {                       // the receiver is up when the packet arrives
             Rec q;
-            unpack(p.rec[2 * iv], p.rec[2 * iv + 1], q);
+            unpack(load_rec(p.rec, (size_t)s * p.stride + dl), q);
             flag |= byz_anomalous(q, e, p.delta);
           }
         }

@@ -25,7 +25,16 @@
 //                         LeaveMessage.prune (types/leave.rs:39-44)
 //   30 u16 conf_mask      suspicion confirmer buckets (Lifeguard)
 #pragma once
+#include <cstddef>
 #include <cstdint>
+
+// Small format and rule helpers are force-inlined under nvcc, as the kernel code they serve: the tick kernels' machine code
+// depends on the point at which a helper is inlined.
+#ifdef __CUDACC__
+#define SFS_HD __host__ __device__ __forceinline__
+#else
+#define SFS_HD inline
+#endif
 
 namespace sfs {
 
@@ -51,38 +60,53 @@ constexpr u32 INC_LIMIT = (1u << 26) - 16;
 
 // node_state word: bits 0-31 LamportClock (types/clock.rs:125), 32 up, 40-41 SerfState
 constexpr u64 NS_UP = 1ull << 32;
+SFS_HD u64 node_word(u32 clock, bool up, u32 sstate) { return (u64)clock | (up ? NS_UP : 0) | ((u64)sstate << 40); }
+SFS_HD u32 nw_clock(u64 ns) { return (u32)ns; }
+SFS_HD bool nw_up(u64 ns) { return (ns & NS_UP) != 0; }
+SFS_HD u32 nw_sstate(u64 ns) { return (u32)(ns >> 40) & 3; }
+
+// busy byte of a node: bit 0 awake (queued transmits / probe duty), bit 1 host operation this tick, bit 2 watcher (static),
+// bit 3 some view of the node runs a suspicion timer (it sleeps until its tile comes due, tick_kernel.cuh)
+constexpr u32 BUSY_AWAKE = 1u, BUSY_OP = 2u, BUSY_WATCH = 4u, BUSY_TIMER = 8u;
 
 struct Rec {
   u32 st, qjoin, qleave, inc, deadline, leave_tick;
   u32 status, mlstate, qfrom, txj, txl, txm, flags, mask;
 };
 
-__host__ __device__ inline void unpack(const uint4& a, const uint4& b, Rec& r) {
-  r.st = a.x; r.qjoin = a.y; r.qleave = a.z; r.inc = a.w;
-  r.deadline = b.x; r.leave_tick = b.y;
-  r.status = b.z & 0xff; r.mlstate = (b.z >> 8) & 3; r.qfrom = (b.z >> 10) & 15;
-  r.txj = (b.z >> 16) & 0xff; r.txl = b.z >> 24;
-  r.txm = b.w & 0xff; r.flags = (b.w >> 8) & 0xff; r.mask = b.w >> 16;
+// The 32-byte image of a record as eight words (layout above).  In memory a record is two uint4 (one sector).
+struct Words { u32 w[8]; };
+SFS_HD Words rec_words(const uint4& a, const uint4& b) { return Words{{a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}}; }
+SFS_HD Words load_rec(const uint4* rec, size_t i) { return rec_words(rec[2 * i], rec[2 * i + 1]); }
+SFS_HD void store_rec(uint4* rec, size_t i, const Words& x) {
+  rec[2 * i] = uint4{x.w[0], x.w[1], x.w[2], x.w[3]}; rec[2 * i + 1] = uint4{x.w[4], x.w[5], x.w[6], x.w[7]};
 }
-__host__ __device__ inline void pack(const Rec& r, uint4& a, uint4& b) {
-  a.x = r.st; a.y = r.qjoin; a.z = r.qleave; a.w = r.inc;
-  b.x = r.deadline; b.y = r.leave_tick;
-  b.z = r.status | (r.mlstate << 8) | (r.qfrom << 10) | (r.txj << 16) | (r.txl << 24);
-  b.w = r.txm | (r.flags << 8) | (r.mask << 16);
+SFS_HD bool differs(const Words& a, const Words& b) {
+  return ((a.w[0] ^ b.w[0]) | (a.w[1] ^ b.w[1]) | (a.w[2] ^ b.w[2]) | (a.w[3] ^ b.w[3]) | (a.w[4] ^ b.w[4]) | (a.w[5] ^ b.w[5]) | (a.w[6] ^ b.w[6]) | (a.w[7] ^ b.w[7])) != 0;
+}
+
+SFS_HD void unpack(const Words& x, Rec& r) {
+  r.st = x.w[0]; r.qjoin = x.w[1]; r.qleave = x.w[2]; r.inc = x.w[3]; r.deadline = x.w[4]; r.leave_tick = x.w[5];
+  r.status = x.w[6] & 0xff; r.mlstate = (x.w[6] >> 8) & 3; r.qfrom = (x.w[6] >> 10) & 15; r.txj = (x.w[6] >> 16) & 0xff; r.txl = x.w[6] >> 24;
+  r.txm = x.w[7] & 0xff; r.flags = (x.w[7] >> 8) & 0xff; r.mask = x.w[7] >> 16;
+}
+SFS_HD void unpack(const uint4& a, const uint4& b, Rec& r) { unpack(rec_words(a, b), r); }   // a record as its two halves in memory
+SFS_HD void pack(const Rec& r, Words& x) {
+  x.w[0] = r.st; x.w[1] = r.qjoin; x.w[2] = r.qleave; x.w[3] = r.inc; x.w[4] = r.deadline; x.w[5] = r.leave_tick;
+  x.w[6] = r.status | (r.mlstate << 8) | (r.qfrom << 10) | (r.txj << 16) | (r.txl << 24);
+  x.w[7] = r.txm | (r.flags << 8) | (r.mask << 16);
 }
 
 // Queue word: the three transmit budgets of a view live in their own 4-byte plane (byte 0 tx_join, 1 tx_leave, 2 tx_ml),
 // so that a sender which only decrements budgets rewrites 4 bytes instead of its whole 32-byte record.  Every external
 // image of a record (records getter, state hash, oracle comparison) is the MERGED one: record | budgets.
-__host__ __device__ inline void merge_queue_word(uint4& b, u32 q) {
-  b.z |= ((q & 0xffu) << 16) | (((q >> 8) & 0xffu) << 24);
-  b.w |= (q >> 16) & 0xffu;
-}
-__host__ __device__ inline u32 split_queue_word(uint4& b) {
-  const u32 q = ((b.z >> 16) & 0xffu) | ((b.z >> 24) << 8) | ((b.w & 0xffu) << 16);
-  b.z &= 0x0000ffffu; b.w &= ~0xffu;
+SFS_HD void merge_queue_word(Words& x, u32 q) { x.w[6] |= ((q & 0xffu) << 16) | (((q >> 8) & 0xffu) << 24); x.w[7] |= (q >> 16) & 0xffu; }
+SFS_HD u32 split_queue_word(Words& x) {
+  const u32 q = ((x.w[6] >> 16) & 0xffu) | ((x.w[6] >> 24) << 8) | ((x.w[7] & 0xffu) << 16);
+  x.w[6] &= 0x0000ffffu; x.w[7] &= ~0xffu;
   return q;
 }
+SFS_HD bool rec_queued(const Rec& r) { return (r.txl | r.txj | r.txm) != 0; }
 
 struct Rules {          // per-run constants
   u32 limit;            // memberlist retransmit limit = retransmit_mult * ceil(log10(n+1))
@@ -94,6 +118,13 @@ struct Rules {          // per-run constants
 __host__ __device__ inline void witness(u32& c, u32 t) { if (t >= c) c = t + 1; }
 
 __host__ __device__ inline u32 from_bucket(u32 node) { return (node * 0x9E3779B1u) >> 28; }
+SFS_HD u32 popc(u32 x) {
+#ifdef __CUDA_ARCH__
+  return (u32)__popc(x);
+#else
+  return (u32)__builtin_popcount(x);
+#endif
+}
 
 // handle_node_join_intent — serf/base.rs:1338-1373 (witness by the caller); re-queue = serf/delegate.rs:294-300
 __host__ __device__ inline void join_intent(Rec& r, u32 lt, u32 limit, bool requeue = true) {
@@ -115,6 +146,8 @@ __host__ __device__ inline void join_intent(Rec& r, u32 lt, u32 limit, bool requ
 // dropped — and at equal Lamport time the intent WITHOUT prune is the greater one, so that applying the greatest alone equals
 // applying all of them in ascending order with the lesser ones' flags dropped.
 __host__ __device__ inline u32 leave_key(u32 lt, bool prune) { return (lt << 1) | (prune ? 0u : 1u); }
+SFS_HD u32 leave_key_lt(u32 key) { return key >> 1; }
+SFS_HD bool leave_key_prune(u32 key) { return !(key & 1u); }
 
 // handle_node_leave_intent — serf/base.rs:1442-1572; prune → handle_prune, :1504-1570, 1628-1653: the member is erased from the
 // view (erase_node!, :499-519).  The reference sleeps broadcast_timeout + leave_propagate_delay first when the member is Leaving,
@@ -172,13 +205,7 @@ __host__ __device__ inline void ml_alive(Rec& r, u32 a, bool self, u32 limit) {
 __host__ __device__ inline void ml_suspect(Rec& r, u32 s, u32 fromb, u32 tick, bool self, const Rules& cx) {
   if (s < r.inc) return;
   if (r.mlstate == ML_SUSPECT) {                                // timer exists → suspicion.Confirm(from)
-    u32 n_old = (u32)
-#ifdef __CUDA_ARCH__
-        __popc(r.mask)
-#else
-        __builtin_popcount(r.mask)
-#endif
-        - 1;
+    u32 n_old = popc(r.mask) - 1;
     if (n_old >= cx.k) return;
     if (r.mask & (1u << fromb)) return;
     r.mask |= (1u << fromb);
@@ -199,7 +226,39 @@ __host__ __device__ inline void ml_dead(Rec& r, u32 d, bool left, u32 tick, bool
   r.inc = d; r.mlstate = left ? ML_LEFT : ML_DEAD; r.qfrom = 0; r.txm = limit;
   node_leave(r, tick);                                          // EventDelegate::notify_leave, serf/delegate.rs:571
 }
+// Memberlist messages on the wire (inbox words, window entries): key = incarnation << 6 | state << 4 | from-bucket.
 __host__ __device__ inline u32 ml_key(const Rec& r) { return (r.inc << 6) | (r.mlstate << 4) | r.qfrom; }
+SFS_HD u32 ml_key_inc(u32 key) { return key >> 6; }
+SFS_HD u32 ml_key_state(u32 key) { return (key >> 4) & 3; }
+SFS_HD u32 ml_key_from(u32 key) { return key & 15; }
+
+// Rules a view is held to after its messages were merged — the tick kernel's node pass and the push-pull round alike.
+// Refutation of a leave intent about ourselves: serf/base.rs:1470-1480 → broadcast_join(clock.time()), :381-397
+SFS_HD void refute_leave(Rec& r, u32& clock, u32 limit) {
+  const u32 T = clock; witness(clock, T);
+  join_intent(r, T, limit);
+  r.qjoin = T; r.txj = limit;
+}
+// A buffered intent that changed gets the tick as its wall time: NodeIntent.wall_time (types/member.rs:32)
+SFS_HD void stamp_intent(Rec& r, const Words& before, u32 tick) {
+  if (!(r.flags & 1) && r.status != TY_NONE && (r.status != (before.w[6] & 0xff) || r.st != before.w[0])) r.leave_tick = tick + 1;
+}
+// Is a watcher's own failed probe still a confirmation (its bucket not in the confirmer set, the set not full)?
+SFS_HD bool can_confirm(u32 k, u32 mask, u32 v) { return popc(mask) - 1u < k && !(mask & (1u << from_bucket(v))); }
+// A watcher of a down subject probes it (wmask: the subjects among the node's neighbours).
+SFS_HD bool view_watching(bool watcher, u32 probe_every, u32 down_mask, u32 s, bool self, u32 wmask) {
+  return watcher && probe_every && ((down_mask >> s) & 1) && !self && ((wmask >> s) & 1);
+}
+// The trace's `pending`: queued transmits, or a watcher that has not noticed yet.  Suspect views are counted apart (they sleep).
+SFS_HD bool view_pending(const Rec& r, bool watching) {
+  return r.mlstate != ML_SUSPECT && (rec_queued(r) || (watching && r.mlstate == ML_ALIVE));
+}
+// Does the view keep its node awake: queued transmits, or a watcher whose own failed probe may still start or confirm the
+// suspicion?  confirm() is can_confirm for this view, asked only of a watched Suspect view.
+template <class Confirm>
+SFS_HD bool view_awake(const Rec& r, bool watching, Confirm confirm) {
+  return rec_queued(r) || (watching && (r.mlstate == ML_ALIVE || (r.mlstate == ML_SUSPECT && confirm())));
+}
 
 // Philox4x32-10 (Salmon et al. 2011): the stateless RNG that picks gossip and probe peers,
 // keyed (seed) and counted (tick, node, block, domain) so any sharding draws the same edges.
@@ -219,6 +278,62 @@ __host__ __device__ inline void philox4x32_10(u32 c0, u32 c1, u32 c2, u32 c3, u3
   }
   out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
+// One uniformly random neighbour slot of a row of `deg` entries (SWIM probe target, push-pull partner).
+SFS_HD u32 neighbour_slot(u32 tick, u32 v, u32 domain, u32 seed_lo, u32 seed_hi, u32 deg) {
+  u32 w[4];
+  philox4x32_10(tick, v, 0, domain, seed_lo, seed_hi, w);
+  return ((w[0] & 0xffffu) * deg) >> 16;
+}
+
+// Gossip peers of one node for one tick — memberlist kRandomNodes (k uniformly random distinct members
+// other than ourselves): m = min(fanout, deg) distinct slots of the node's CSR row, sampled without
+// replacement by rank from ONE Philox4x32-10 block (eight 16-bit draws: low half, then high half of words
+// 0..3): draw k picks rank j = (h16_k·(deg−k)) >> 16 among the slots not chosen yet; slots pointing at the
+// node itself are dropped; peers are used in draw order.  No rejection loop, no divergence, m gathers.
+// Every sender draws its peers this way (membership tick, user events, injectors): they ride in the same packets.
+constexpr u32 NO_TARGET = 0xffffffffu;
+SFS_HD u32 draw16(const u32 (&w)[4], int i) { const u32 x = w[(i >> 1) & 3]; return (i & 1) ? (x >> 16) : (x & 0xffffu); }
+// peer_issue draws the slots and requests the neighbour ids (cand[]: col(row0 + slot), loads in flight, v for an unused draw);
+// peer_finish drops self slots and packs the targets.
+template <int FMAX, class Col>
+SFS_HD void peer_issue(u32 tick, u32 v, u32 fanout, u32 seed_lo, u32 seed_hi, u32 row0, u32 deg, Col col, u32 (&cand)[FMAX]) {
+  const u32 m = fanout < deg ? fanout : deg;
+  u32 w[4];
+  philox4x32_10(tick, v, 0, DOMAIN_GOSSIP, seed_lo, seed_hi, w);
+  u32 srt[FMAX];                                           // chosen slots so far, ascending; unused entries = NO_TARGET (sort last)
+#pragma unroll
+  for (int k = 0; k < FMAX; ++k) srt[k] = NO_TARGET;
+#pragma unroll
+  for (int k = 0; k < FMAX; ++k) {
+    u32 j = (draw16(w, k) * (deg - ((u32)k < deg ? (u32)k : deg))) >> 16;
+#pragma unroll
+    for (int i = 0; i < k; ++i) j += (j >= srt[i]) ? 1u : 0u;         // rank → slot: skip the slots already taken
+    const bool use = (u32)k < m;
+    const u32 e = row0 + (use ? j : 0u);
+    cand[k] = use ? col(e) : v;
+    // insert j into the ascending list (only if used): bubble it down from position k
+    u32 x = use ? j : NO_TARGET;
+#pragma unroll
+    for (int i = 0; i < k; ++i) { const u32 lo = srt[i] < x ? srt[i] : x, hi = srt[i] < x ? x : srt[i]; srt[i] = lo; x = hi; }
+    srt[k] = x;
+  }
+}
+template <int FMAX>
+SFS_HD u32 peer_finish(u32 v, const u32 (&cand)[FMAX], u32 (&tg)[FMAX]) {
+  u32 nt = 0;
+#pragma unroll
+  for (int k = 0; k < FMAX; ++k) tg[k] = NO_TARGET;
+#pragma unroll
+  for (int k = 0; k < FMAX; ++k) {
+    if (cand[k] != v) {                                    // self slots (and the unused tail) are dropped
+#pragma unroll
+      for (int j2 = 0; j2 <= k; ++j2) tg[j2] = ((u32)j2 == nt) ? cand[k] : tg[j2];
+      ++nt;
+    }
+  }
+  return nt;
+}
+
 __host__ __device__ inline u32 mulhi32(u32 a, u32 b) {
 #ifdef __CUDA_ARCH__
   return __umulhi(a, b);
@@ -232,12 +347,12 @@ __host__ __device__ inline u64 mix64(u64 x) {
   x ^= x >> 27; x *= 0x94d049bb133111ebULL;
   x ^= x >> 31; return x;
 }
-__host__ __device__ inline u64 rec_hash(u64 idx, const uint4& a, const uint4& b) {
-  u64 w0 = a.x | ((u64)a.y << 32), w1 = a.z | ((u64)a.w << 32), w2 = b.x | ((u64)b.y << 32), w3 = b.z | ((u64)b.w << 32);
+__host__ __device__ inline u64 rec_hash(u64 idx, const Words& x) {
+  u64 w0 = x.w[0] | ((u64)x.w[1] << 32), w1 = x.w[2] | ((u64)x.w[3] << 32), w2 = x.w[4] | ((u64)x.w[5] << 32), w3 = x.w[6] | ((u64)x.w[7] << 32);
   return mix64(w0 ^ mix64(w1 ^ mix64(w2 ^ mix64(w3 ^ mix64(idx + 0x9e3779b97f4a7c15ULL)))));
 }
 __host__ __device__ inline u64 node_hash(u64 idx, u64 ns) {
-  u64 w = (ns & 0xffffffffull) | (((ns >> 32) & 1) << 32) | (((ns >> 40) & 3) << 40);
+  const u64 w = node_word(nw_clock(ns), nw_up(ns), nw_sstate(ns));
   return mix64(w ^ mix64(idx + 0x9e3779b97f4a7c15ULL));
 }
 

@@ -8,6 +8,7 @@
 // tick_kernel.cu.  There is no CPU execution path: without a CUDA device every entry point fails.
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -20,6 +21,13 @@
 #include "wire.cuh"
 
 using namespace sfs;
+
+// The kernels index a tick's trace row by ROW_* (tick_kernel.cuh); the host hands it out as serfsim_tick_row_t.
+#define SFS_ROW_FIELD(i, f) static_assert(i == offsetof(serfsim_tick_row_t, f) / sizeof(uint64_t), #i " is serfsim_tick_row_t::" #f)
+SFS_ROW_FIELD(ROW_PACKETS, packets); SFS_ROW_FIELD(ROW_EDGES, edge_updates); SFS_ROW_FIELD(ROW_MESSAGES, messages); SFS_ROW_FIELD(ROW_CHANGED, changed);
+SFS_ROW_FIELD(ROW_PENDING, pending); SFS_ROW_FIELD(ROW_EVENTS, events); SFS_ROW_FIELD(ROW_SUSPECTS, suspects); SFS_ROW_FIELD(ROW_HASH, hash);
+#undef SFS_ROW_FIELD
+static_assert(sizeof(serfsim_tick_row_t) == ROW_FIELDS * sizeof(uint64_t), "a trace row is ROW_FIELDS counters");
 
 namespace {
 
@@ -286,18 +294,18 @@ int ensure_trace(serfsim* h, u32 need) {
   while (cap < need) cap *= 2;
   u64* nt = nullptr; u32* nk = nullptr; u32* nv = nullptr; u64* ng = nullptr;
   const bool sharded = h->cfg.world_size > 1;
-  CU(cudaMalloc(&nt, (size_t)cap * 8 * sizeof(u64)));
+  CU(cudaMalloc(&nt, (size_t)cap * sizeof(serfsim_tick_row_t)));
   CU(cudaMalloc(&nk, ((size_t)cap + 1) * 4 * sizeof(u32)));
   CU(cudaMalloc(&nv, ((size_t)cap + 1) * h->R * 4 * sizeof(u32)));
-  CU(cudaMemsetAsync(nt, 0, (size_t)cap * 8 * sizeof(u64), h->stream));
+  CU(cudaMemsetAsync(nt, 0, (size_t)cap * sizeof(serfsim_tick_row_t), h->stream));
   CU(cudaMemsetAsync(nk, 0, ((size_t)cap + 1) * 4 * sizeof(u32), h->stream));
   CU(cudaMemsetAsync(nv, 0, ((size_t)cap + 1) * h->R * 4 * sizeof(u32), h->stream));
-  if (sharded) { CU(cudaMalloc(&ng, (size_t)cap * 8 * sizeof(u64))); CU(cudaMemsetAsync(ng, 0, (size_t)cap * 8 * sizeof(u64), h->stream)); }
+  if (sharded) { CU(cudaMalloc(&ng, (size_t)cap * sizeof(serfsim_tick_row_t))); CU(cudaMemsetAsync(ng, 0, (size_t)cap * sizeof(serfsim_tick_row_t), h->stream)); }
   if (h->d_trace) {
-    CU(cudaMemcpyAsync(nt, h->d_trace, (size_t)h->trace_cap * 8 * sizeof(u64), cudaMemcpyDeviceToDevice, h->stream));
+    CU(cudaMemcpyAsync(nt, h->d_trace, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToDevice, h->stream));
     CU(cudaMemcpyAsync(nk, h->d_kinds, ((size_t)h->trace_cap + 1) * 4 * sizeof(u32), cudaMemcpyDeviceToDevice, h->stream));
     CU(cudaMemcpyAsync(nv, h->d_view_kinds, ((size_t)h->trace_cap + 1) * h->R * 4 * sizeof(u32), cudaMemcpyDeviceToDevice, h->stream));
-    if (sharded) CU(cudaMemcpyAsync(ng, h->d_grow, (size_t)h->trace_cap * 8 * sizeof(u64), cudaMemcpyDeviceToDevice, h->stream));
+    if (sharded) CU(cudaMemcpyAsync(ng, h->d_grow, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToDevice, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds); cudaFree(h->d_grow);
   }
@@ -424,7 +432,7 @@ TickParams tick_params(const serfsim* h, u32 t, OpRange ops) {
   p.rec = h->d_rec; p.qword = h->d_qword; p.inbox_rd = h->d_inbox[(t & 1) ^ 1]; p.inbox_wr = h->d_inbox[t & 1];
   p.node_state = h->d_node; p.busy = h->d_busy; p.watch = h->d_watch; p.row_ptr = h->d_rowptr; p.col = h->d_col;
   p.ev_node = h->d_ev_node; p.ev_op = h->d_ev_op; p.ev_slot = h->d_ev_slot;
-  p.row = h->d_trace + (size_t)t * 8;
+  p.row = h->d_trace + (size_t)t * ROW_FIELDS;
   p.kinds_prev = h->d_kinds + (size_t)t * 4;
   p.kinds_cur = h->d_kinds + ((size_t)t + 1) * 4;
   p.overflow = h->d_overflow;
@@ -447,11 +455,11 @@ TickParams tick_params(const serfsim* h, u32 t, OpRange ops) {
   p.win_data = h->d_peer_data[xpar]; p.send_count = h->d_send_count;
   p.peer_ctrl = h->d_peer_ctrl; p.stamp = h->xepoch + 1; p.xpar = xpar; p.loopback = h->loopback ? 1u : 0u;
   p.fuse_publish = (sharded && !h->byz_on && !h->sw.no_fuse) ? 1u : 0u;
-  p.shard_inv = (u32)(0x100000000ull / h->shard_size); p.xcap = p.world > 1 ? 392u / (p.world - 1) : 0u;     // XW_TOTAL = 392 (tick_kernel.cu)
+  p.shard_inv = (u32)(0x100000000ull / h->shard_size); p.xcap = p.world > 1 ? XW_TOTAL / (p.world - 1) : 0u;
   if (h->gate_on) {                                // convergence gate: the first kernel of the tick evaluates the row of tick t-1
     const u64* grow = sharded ? h->d_grow : h->d_trace;            // global rows: the device sums them when sharded
     Gate& g = p.gate;
-    g.ctl = h->d_runctl; g.host_ctl = h->d_pin_ctl; g.prev_row = t > h->gate_first ? grow + (size_t)(t - 1) * 8 : nullptr; g.tick = t;
+    g.ctl = h->d_runctl; g.host_ctl = h->d_pin_ctl; g.prev_row = t > h->gate_first ? grow + (size_t)(t - 1) * ROW_FIELDS : nullptr; g.tick = t;
     g.future_ops = (t > 0 && future_ops(h, t - 1)) ? 1u : 0u;
     g.pp = p.pp_every; g.byz_on = h->byz_on ? 1u : 0u;
   }
@@ -537,7 +545,7 @@ void launch_exchange(serfsim* h, const TickParams& p) {
   d.win_data = h->d_win_data[xpar]; d.ctrl = h->d_ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
   d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = h->d_peer_anomaly;
   d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->d_ue_inbox[t & 1] : nullptr; d.ue_ltime = h->d_ue_ltime;
-  d.my_row = p.row; d.grow = h->d_grow + (size_t)t * 8; d.gate = p.gate.ctl;
+  d.my_row = p.row; d.grow = h->d_grow + (size_t)t * ROW_FIELDS; d.gate = p.gate.ctl;
   d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(h->d_ctrl) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
   d.sched = h->d_sched; d.sched_rw = h->d_sched; d.host_idle_until = h->d_pin_ctl + 2; d.tick = t; d.sleep_on = p.sleep_on;
   launch_drain(d, h->stream);
@@ -577,10 +585,10 @@ int anti_entropy_round(serfsim* h, TickParams p) {
     h->barrier(h->comm_user);
     // the round changed this rank's row (changed / pending / hash) after the drain kernel summed the rows: redo the sum through
     // the host hook — the host is in the loop here anyway (two barriers), and rounds are rare
-    u64 row[8];
-    CU(cudaMemcpy(row, h->d_trace + (size_t)t * 8, sizeof(row), cudaMemcpyDeviceToHost));
-    h->allreduce(h->comm_user, row, 8);
-    CU(cudaMemcpy(h->d_grow + (size_t)t * 8, row, sizeof(row), cudaMemcpyHostToDevice));
+    u64 row[ROW_FIELDS];
+    CU(cudaMemcpy(row, h->d_trace + (size_t)t * ROW_FIELDS, sizeof(row), cudaMemcpyDeviceToHost));
+    h->allreduce(h->comm_user, row, ROW_FIELDS);
+    CU(cudaMemcpy(h->d_grow + (size_t)t * ROW_FIELDS, row, sizeof(row), cudaMemcpyHostToDevice));
   } else {
     launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
   }
@@ -681,7 +689,7 @@ int pull_rows(serfsim* h) {                     // bring rows [rows.size(), tick
   h->rows.resize(h->tick);
   // sharded runs: the drain kernel of every tick has already summed the ranks' rows on the device (d_grow), no host collective
   const u64* src = h->cfg.world_size > 1 ? h->d_grow : h->d_trace;
-  CU(cudaMemcpy(h->rows.data() + have, src + (size_t)have * 8, (size_t)n * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(h->rows.data() + have, src + (size_t)have * ROW_FIELDS, (size_t)n * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -749,11 +757,11 @@ int do_reset(serfsim* h, u64 seed) {
   if (h->d_carry) CU(cudaMemsetAsync(h->d_carry, 0, (size_t)h->stride * sizeof(u32), h->stream));   // tags restart with the ticks
   CU(cudaMemsetAsync(h->d_sched, 0, SCHED_WORDS * sizeof(u32), h->stream));
   if (h->d_trace) {
-    CU(cudaMemsetAsync(h->d_trace, 0, (size_t)h->trace_cap * 8 * sizeof(u64), h->stream));
+    CU(cudaMemsetAsync(h->d_trace, 0, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), h->stream));
     CU(cudaMemsetAsync(h->d_kinds, 0, ((size_t)h->trace_cap + 1) * 4 * sizeof(u32), h->stream));
     CU(cudaMemsetAsync(h->d_view_kinds, 0, ((size_t)h->trace_cap + 1) * h->R * 4 * sizeof(u32), h->stream));
   }
-  if (h->d_grow) CU(cudaMemsetAsync(h->d_grow, 0, (size_t)h->trace_cap * 8 * sizeof(u64), h->stream));
+  if (h->d_grow) CU(cudaMemsetAsync(h->d_grow, 0, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), h->stream));
   CU(cudaMemsetAsync(h->d_runctl, 0, 2 * sizeof(u32), h->stream));
   if (h->d_send_count) CU(cudaMemsetAsync(h->d_send_count, 0, sizeof(u32) * 8, h->stream));
   { int rc = ue_reset(h); if (rc) return rc; }
@@ -898,7 +906,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
 #define CUB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return bail(fail(e_ == cudaErrorMemoryAllocation ? SERFSIM_E_NOMEM : SERFSIM_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_))); } while (0)
   CUB(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   CUB(cudaEventCreate(&h->ev0)); CUB(cudaEventCreate(&h->ev1));
-  h->stride = ((h->count + 255) / 256) * 256;
+  h->stride = plane_stride(h->count);
   const size_t inbox_bytes = (size_t)3 * h->R * h->stride * sizeof(u32);
   CUB(cudaMalloc(&h->d_rec, (size_t)h->R * h->stride * 32));
   CUB(cudaMemset(h->d_rec, 0, (size_t)h->R * h->stride * 32));
@@ -907,7 +915,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   CUB(cudaMalloc(&h->d_inbox[0], inbox_bytes)); CUB(cudaMalloc(&h->d_inbox[1], inbox_bytes));
   CUB(cudaMalloc(&h->d_node, (size_t)h->stride * 8));
   CUB(cudaMemset(h->d_node, 0, (size_t)h->stride * 8));
-  h->n_tiles = (h->count + 255) / 256;
+  h->n_tiles = h->stride >> TILE_SHIFT;
   CUB(cudaMalloc(&h->d_busy, h->stride));
   CUB(cudaMalloc(&h->d_watch, (size_t)h->stride * 2));
   CUB(cudaMemset(h->d_watch, 0, (size_t)h->stride * 2));
@@ -945,8 +953,8 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   if (cfg->world_size > 1) {
     // receive windows: one segment per peer; expected entries per tick and pair ≈ shard · fanout · R · kinds / world
     if (cfg->world_size > 8) return bail(fail(SERFSIM_E_INVAL, "world_size > 8"));
-    // … plus the entries the warps of the tick kernel reserve ahead and do not fill (flush_xwarp: at most XW_RESERVE_MAX = 128 per warp and peer)
-    const double pad = (double)std::max(h->grid, h->grid_sv) * 8.0 * 160.0;   // (the single-view kernel of a multi-slot run has the larger grid)
+    // … plus what a warp of the tick kernel (TILE threads) can leave unfilled in a peer's window: its reservation ahead and a partial block
+    const double pad = (double)std::max(h->grid, h->grid_sv) * (TILE / 32) * (XW_RESERVE_MAX + XW_FLUSH);   // (the single-view kernel of a multi-slot run has the larger grid)
     double cap = (double)h->shard_size * cfg->fanout * h->R * 3.0 * h->sw.win_factor / cfg->world_size + 4096.0 + pad;
     h->win_cap = (u32)std::min(cap, 4.0e9);
     h->win_cap_base = h->win_cap;

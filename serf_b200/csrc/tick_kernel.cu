@@ -43,17 +43,14 @@ constexpr int BLOCK = 256;
 #ifndef SFS_MB_RN
 #define SFS_MB_RN 1                         // multi-slot kernels (up to 255 registers per thread; ptxas uses about 200)
 #endif
-constexpr u32 TILE_SHIFT = 8;              // one tile = one CTA pass = 256 nodes
 constexpr u32 MAX_TILES_PER_CTA = 1024;
-static_assert((1u << TILE_SHIFT) == BLOCK, "tile = block");
+static_assert(TILE == BLOCK, "tile = block");
 
 // ---- cache-policy plumbing -------------------------------------------------------------------
 // The only randomly addressed data of a tick are the inbox planes the sends reduce into (RED.MAX,
 // 4 B at a random node).  They are kept L2-resident with an evict_last policy; everything that is
 // streamed exactly once per tick (records, node state, the inbox parity being consumed) goes
 // through evict_first / no-L1-allocate so it does not push the inbox out of the 50 MB L2.
-struct Words { u32 w[8]; };   // one 32-byte record
-
 #ifndef SERFSIM_EMU
 __device__ __forceinline__ u64 policy_evict_first() { u64 p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p; }
 __device__ __forceinline__ u64 policy_evict_last() { u64 p; asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p; }
@@ -174,8 +171,6 @@ __device__ __forceinline__ u64 warp_sum64(u64 v) {
 // window by its own warp — 256+ contiguous bytes over NVLink, one global counter atomic per flush, no CTA barrier
 // anywhere (a per-tile CTA-wide flush cost four barriers per tile and made every warp wait for the slowest one).
 constexpr u32 MAX_WORLD = 8;
-constexpr u32 XW_TOTAL = 392;              // staged entries per warp (3 KB), split evenly over the world-1 peers (world 8: 56 each)
-constexpr u32 XW_FLUSH = 32;               // flush threshold: a full warp-wide store
 struct XStage { u64 buf[(BLOCK / 32) * XW_TOTAL]; u32 cnt[BLOCK / 32][MAX_WORLD]; };
 // (no integer division on the send path: the sharded kernel issues on every cycle it can — 2.4× the instructions of the unsharded one —
 // and `x / runtime value` is ≈ 25 of them; capacity and reciprocal come with the parameters)
@@ -202,7 +197,7 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
   } else {
     u32 dloc;
     const u32 shard = shard_of(p, dst, dloc);
-    const u64 e = ((u64)val1 << 32) | ((u64)(s + p.sv_wshift) << 28) | ((u64)kind << 26) | dloc;   // (a single-view launch numbers its view 0: the entry carries the real one)
+    const u64 e = win_entry(val1, s + p.sv_wshift, kind, dloc);   // (a single-view launch numbers its view 0: the entry carries the real one)
     // warp-aggregated append: the lanes of this call that target the same shard reserve their slots with ONE
     // shared-memory atomic on the warp's own counter (divergent callers of the same warp may interleave: keep it atomic)
 #ifdef SFS_XSTAGE_MATCH                           // A/B: one shared atomic per distinct shard of the call (match_any + leader + shuffle)
@@ -219,9 +214,7 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
     if (pos < xcap(p)) {
       xs->buf[wid * XW_TOTAL + xseg(p, shard) + pos] = e;
     } else {                                   // buffer full: write this one straight through
-      const u32 g = atomicAdd(p.send_count + shard, 1u);
-      if (g < p.win_cap) p.win_data[shard][(size_t)p.rank * p.win_cap + g] = e;
-      else *p.overflow = 2;
+      win_append<1>(p, shard, {e});
     }
   }
 }
@@ -249,7 +242,6 @@ __device__ __forceinline__ void send_deduped(const TickParams& p, u32* plane, co
 // made when the kernel starts.  A flush that needs more than it holds takes the rest synchronously.  Reserved entries that stay
 // unwritten read as zeros at the receiver: the drain kernel skips zero entries and clears every entry it consumes, so a window
 // is all zeros again before it is written next.  force = false: whole blocks only; force = true (end of the kernel): everything.
-constexpr u32 XW_RESERVE_MAX = 128;        // entries reserved ahead per warp and peer, at most (bounds the padding, serfsim_create)
 __device__ __forceinline__ bool flush_xwarp(const TickParams& p, XStage* xs, bool force, u32& resv, u32& rlen) {
   const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   __syncwarp();
@@ -297,79 +289,18 @@ __device__ __forceinline__ bool flush_xwarp(const TickParams& p, XStage* xs, boo
   return wrote;
 }
 
-__device__ __forceinline__ void unpack_words(const Words& x, Rec& r) {
-  r.st = x.w[0]; r.qjoin = x.w[1]; r.qleave = x.w[2]; r.inc = x.w[3]; r.deadline = x.w[4]; r.leave_tick = x.w[5];
-  r.status = x.w[6] & 0xff; r.mlstate = (x.w[6] >> 8) & 3; r.qfrom = (x.w[6] >> 10) & 15; r.txj = (x.w[6] >> 16) & 0xff; r.txl = x.w[6] >> 24;
-  r.txm = x.w[7] & 0xff; r.flags = (x.w[7] >> 8) & 0xff; r.mask = x.w[7] >> 16;
-}
-__device__ __forceinline__ void pack_words(const Rec& r, Words& x) {
-  x.w[0] = r.st; x.w[1] = r.qjoin; x.w[2] = r.qleave; x.w[3] = r.inc; x.w[4] = r.deadline; x.w[5] = r.leave_tick;
-  x.w[6] = r.status | (r.mlstate << 8) | (r.qfrom << 10) | (r.txj << 16) | (r.txl << 24);
-  x.w[7] = r.txm | (r.flags << 8) | (r.mask << 16);
-}
-__device__ __forceinline__ void merge_q(Words& x, u32 q) { x.w[6] |= ((q & 0xffu) << 16) | (((q >> 8) & 0xffu) << 24); x.w[7] |= (q >> 16) & 0xffu; }
-__device__ __forceinline__ u32 split_q(Words& x) {
-  const u32 q = ((x.w[6] >> 16) & 0xffu) | ((x.w[6] >> 24) << 8) | ((x.w[7] & 0xffu) << 16);
-  x.w[6] &= 0x0000ffffu; x.w[7] &= ~0xffu;
-  return q;
-}
-__device__ __forceinline__ bool differs(const Words& a, const Words& b) {
-  return ((a.w[0] ^ b.w[0]) | (a.w[1] ^ b.w[1]) | (a.w[2] ^ b.w[2]) | (a.w[3] ^ b.w[3]) | (a.w[4] ^ b.w[4]) | (a.w[5] ^ b.w[5]) | (a.w[6] ^ b.w[6]) | (a.w[7] ^ b.w[7])) != 0;
-}
-
-// Gossip peers of one node for one tick — memberlist kRandomNodes (k uniformly random distinct members
-// other than ourselves): m = min(fanout, deg) distinct slots of the node's CSR row, sampled without
-// replacement by rank from ONE Philox4x32-10 block (eight 16-bit draws: low half, then high half of words
-// 0..3): draw k picks rank j = (h16_k·(deg−k)) >> 16 among the slots not chosen yet; slots pointing at the
-// node itself are dropped; peers are used in draw order.  No rejection loop, no divergence, m gathers.
-constexpr u32 NO_TARGET = 0xffffffffu;
-__device__ __forceinline__ u32 draw16(const u32 (&w)[4], int i) { const u32 x = w[(i >> 1) & 3]; return (i & 1) ? (x >> 16) : (x & 0xffffu); }
-// pick_issue draws the slots and requests the neighbour ids (cand[]: loads in flight), pick_finish drops self slots and packs the targets.
+// The gossip peer draw (record.cuh peer_issue) with the neighbour ids requested from the tile's stage or global memory.
 #define SFS_LD_COL(ptr, pol) __ldg(ptr)     // read-only path WITH L1 allocation: the four picks of a node fall into its two CSR sectors, later picks hit L1 (an evict_first / no-allocate gather was 6 % slower in plateau ticks)
 template <int FMAX, bool STAGED>
 __device__ __forceinline__ void pick_issue(const TickParams& p, const StageView& sv, u32 v, u32 row0, u32 deg, u64 pol_first, u32 (&cand)[FMAX]) {
-  const u32 m = min(p.fanout, deg);
-  u32 w[4];
-  philox4x32_10(p.tick, v, 0, DOMAIN_GOSSIP, p.seed_lo, p.seed_hi, w);
-  u32 srt[FMAX];                                           // chosen slots so far, ascending; unused entries = NO_TARGET (sort last)
-#pragma unroll
-  for (int k = 0; k < FMAX; ++k) srt[k] = NO_TARGET;
-#pragma unroll
-  for (int k = 0; k < FMAX; ++k) {
-    u32 j = (draw16(w, k) * (deg - min((u32)k, deg))) >> 16;
-#pragma unroll
-    for (int i = 0; i < k; ++i) j += (j >= srt[i]) ? 1u : 0u;         // rank → slot: skip the slots already taken
-    const bool use = (u32)k < m;
-    const u32 e = row0 + (use ? j : 0u);
-    cand[k] = use ? ((STAGED && sv.col_staged) ? sv.col[e - sv.col_base] : SFS_LD_COL(p.col + e, pol_first)) : v;
-    // insert j into the ascending list (only if used): bubble it down from position k
-    u32 x = use ? j : NO_TARGET;
-#pragma unroll
-    for (int i = 0; i < k; ++i) { const u32 lo = min(srt[i], x), hi = max(srt[i], x); srt[i] = lo; x = hi; }
-    srt[k] = x;
-  }
-}
-template <int FMAX>
-__device__ __forceinline__ u32 pick_finish(u32 v, const u32 (&cand)[FMAX], u32 (&tg)[FMAX]) {
-  u32 nt = 0;
-#pragma unroll
-  for (int k = 0; k < FMAX; ++k) tg[k] = NO_TARGET;
-#pragma unroll
-  for (int k = 0; k < FMAX; ++k) {
-    if (cand[k] != v) {                                    // self slots (and the unused tail) are dropped
-#pragma unroll
-      for (int j2 = 0; j2 <= k; ++j2) tg[j2] = ((u32)j2 == nt) ? cand[k] : tg[j2];
-      ++nt;
-    }
-  }
-  return nt;
+  peer_issue<FMAX>(p.tick, v, p.fanout, p.seed_lo, p.seed_hi, row0, deg,
+                   [&](u32 e) { return (STAGED && sv.col_staged) ? sv.col[e - sv.col_base] : SFS_LD_COL(p.col + e, pol_first); }, cand);
 }
 
 // What decides whether a node has anything to do this tick: its busy byte and the inbox words of the previous tick
 // (slot 0 kept; per slot one "has mail" bit), plus — multi-slot runs — one "has queued transmits" bit per slot from the
 // queue words.  13 bytes per node instead of 45 (single slot).
-// busy byte: bit 0 awake (queued transmits / probe duty), bit 1 host operation this tick, bit 2 watcher (static),
-// bit 3 some view of the node runs a suspicion timer (it sleeps until its tile comes due, tick_kernel.cuh).
+// (busy byte: BUSY_*, record.cuh)
 // nd: the node's own earliest suspicion deadline (node_due), read only in tiles that have come due
 struct Pre { u32 busy, mL, mJ, mM, any, qw, mailmask, qmask, keep, nd; };   // mL, mJ, mM, qw: the words of view `keep` (0 in single-slot runs)
 // Carry word of node vl in this tick (CARRY_*), 0 when no earlier pass of the tick visited it.
@@ -411,10 +342,10 @@ __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool k
 // no host operation and no timer due has nothing to do: the view loop leaves it unvisited too.  So a pass skips the nodes that are
 // awake only for another view's sake (in a tick in which one view's wave keeps nearly every node awake, nearly all of them).
 template <bool PASS = false>
-__device__ __forceinline__ u32 busy_business(u32 busy) { return busy & (PASS ? 6u : 7u); }
+__device__ __forceinline__ u32 busy_business(u32 busy) { return busy & (BUSY_OP | BUSY_WATCH | (PASS ? 0u : BUSY_AWAKE)); }
 template <bool PASS = false>
 __device__ __forceinline__ bool node_active(const TickParams& p, const Pre& x, bool due) {
-  return busy_business<PASS>(x.busy) != 0 || x.any != 0 || p.reap_now != 0 || (due && (x.busy & 8u) && x.nd <= p.tick);
+  return busy_business<PASS>(x.busy) != 0 || x.any != 0 || p.reap_now != 0 || (due && (x.busy & BUSY_TIMER) && x.nd <= p.tick);
 }
 
 // Multi-slot runs, saturated ticks: what a node needs beyond its `Pre` words, requested ONE TILE AHEAD together with them — the node
@@ -426,7 +357,7 @@ __device__ __forceinline__ bool node_active(const TickParams& p, const Pre& x, b
 template <int FMAX>
 struct Ahead { u64 ns; Words rec; u32 cand[FMAX]; u32 valid; };
 
-__device__ __forceinline__ u32 sleeping_deadline(const Pre& x, bool due) { return (due && (x.busy & 8u)) ? x.nd : NO_DEADLINE; }
+__device__ __forceinline__ u32 sleeping_deadline(const Pre& x, bool due) { return (due && (x.busy & BUSY_TIMER)) ? x.nd : NO_DEADLINE; }
 
 // ---- cold paths of a node's tick, kept out of line: host operations, the reaper round and the SWIM probe run for a handful of
 // nodes per tick (or for all of them once in a long while); inlined, their temporaries (a second Philox block, the operation
@@ -468,12 +399,10 @@ __device__ SFS_COLD void cold_host_op(Rec& r, u32& clock, u32& sstate, u32 op, b
     if (rf) { const u32 T2 = clock; witness(clock, T2); join_intent(r, T2, limit); r.qjoin = T2; r.txj = limit; }
   }
 }
-// Which host operation targets node v this tick (the mark kernel set bit 1 of its busy byte)?
+// Which host operation targets node v this tick?
 __device__ SFS_COLD u32 cold_find_op(const TickParams& p, u32 v, u32& op_slot) {
-  atomicAdd((unsigned long long*)(p.row + 5), 1ull);
-  for (u32 e = p.ev_begin; e < p.ev_end; ++e)
-    if (p.ev_node[e] == v) { op_slot = p.ev_slot[e]; return p.ev_op[e]; }
-  return 0;
+  atomicAdd((unsigned long long*)(p.row + ROW_EVENTS), 1ull);
+  return host_op_of(p, v, op_slot);
 }
 // Reaper round (serf/base.rs:483-610): Left / Failed members past their timeouts are erased, stale buffered intents dropped.
 __device__ SFS_COLD void cold_reap(Rec& r, u32 t, u32 tombstone, u32 reconnect, u32 intent) {
@@ -487,27 +416,18 @@ __device__ SFS_COLD void cold_reap(Rec& r, u32 t, u32 tombstone, u32 reconnect, 
 }
 // SWIM probe target of a watcher's round: a uniformly random neighbour (memberlist walks a shuffled list).
 __device__ SFS_COLD u32 cold_probe_target(const TickParams& p, u32 v, u32 row0, u32 deg) {
-  u32 w[4];
-  philox4x32_10(p.tick, v, 0, DOMAIN_PROBE, p.seed_lo, p.seed_hi, w);
-  return __ldg(p.col + row0 + (((w[0] & 0xffffu) * deg) >> 16));
+  return __ldg(p.col + row0 + neighbour_slot(p.tick, v, DOMAIN_PROBE, p.seed_lo, p.seed_hi, deg));
 }
 // The probe found the subject down: suspect it (or confirm with this node's bucket).
 __device__ SFS_COLD void cold_probe_hit(const TickParams& p, Rec& r, u32 v) {
   if (r.mlstate == ML_ALIVE || r.mlstate == ML_SUSPECT) {
-    if (r.mlstate == ML_ALIVE) atomicAdd((unsigned long long*)(p.row + 6), 1ull);
+    if (r.mlstate == ML_ALIVE) atomicAdd((unsigned long long*)(p.row + ROW_SUSPECTS), 1ull);
     ml_suspect(r, r.inc, from_bucket(v), p.tick, false, p.rules);
   }
 }
-// Refutation of a leave intent about ourselves: serf/base.rs:1470-1480 → broadcast_join(clock.time()), :381-397
-__device__ SFS_COLD void cold_refute(Rec& r, u32& clock, u32 limit) {
-  const u32 T = clock; witness(clock, T);
-  join_intent(r, T, limit);
-  r.qjoin = T; r.txj = limit;
-}
-// Is a watcher's own failed probe still a confirmation (its bucket not in the confirmer set, the set not full)?
-__device__ SFS_COLD bool cold_can_confirm(u32 k, u32 mask, u32 v) {
-  return (u32)__popc(mask) - 1u < k && !(mask & (1u << from_bucket(v)));
-}
+// The view rules of record.cuh that only a few views need in a tick
+__device__ SFS_COLD void cold_refute(Rec& r, u32& clock, u32 limit) { refute_leave(r, clock, limit); }
+__device__ SFS_COLD bool cold_can_confirm(u32 k, u32 mask, u32 v) { return can_confirm(k, mask, v); }
 
 // Returns true when the node stays awake (queued transmits, probe duty): that keeps its tile hot for the next tick.
 // A view whose only business is a running suspicion timer does not: its deadline goes to `mind` (the caller registers the
@@ -547,7 +467,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
     } else {
       cur = ld_rec256(p.rec + 2 * (size_t)vl, pol_first);
     }
-    merge_q(cur, pre.qw);                                  // the record image everything below works on is record | budgets
+    merge_queue_word(cur, pre.qw);                         // the record image everything below works on is record | budgets
   };
   if (upfront) { load_node(); load_rec0(); }
   const u32 busy = pre.busy;
@@ -556,28 +476,28 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
 
   // ---- idle exit: nothing received (any slot), nothing queued, no host operation, no probe duty, no timer due ----
   u32 nd = pre.nd;                                       // the node's own earliest deadline: matters in due tiles, for nodes that run timers
-  if (R1 && due && (busy & 8u)) nd = p.node_due[vl];
-  const u32 sleeping = (due && (busy & 8u)) ? nd : NO_DEADLINE;
+  if (R1 && due && (busy & BUSY_TIMER)) nd = p.node_due[vl];
+  const u32 sleeping = (due && (busy & BUSY_TIMER)) ? nd : NO_DEADLINE;
   bool timers_due = sleeping <= p.tick;
   u32 cr = 0;                                            // PASS: what the earlier passes of this tick did at this node
   if (PASS && due) { cr = carry_of(p, vl); if (cr & CARRY_SEEN) timers_due = (cr & CARRY_TDUE) != 0; }   // as it was when the tick began
-  if (!TRACE && !STAGED && !(busy_business<PASS>(busy) != 0 || pre.any != 0 || p.reap_now != 0 || timers_due)) { mind = min(mind, sleeping); if (due && (busy & 8u)) SFS_PROBE(20); return false; }
+  if (!TRACE && !STAGED && !(busy_business<PASS>(busy) != 0 || pre.any != 0 || p.reap_now != 0 || timers_due)) { mind = min(mind, sleeping); if (due && (busy & BUSY_TIMER)) SFS_PROBE(20); return false; }
   if (PASS && !due) cr = carry_of(p, vl);
-  if (STAGED && !TRACE && !((busy & 7u) || (mL | mJ | mM) || p.reap_now || timers_due)) { mind = min(mind, sleeping); return false; }
+  if (STAGED && !TRACE && !(busy_business(busy) || (mL | mJ | mM) || p.reap_now || timers_due)) { mind = min(mind, sleeping); return false; }
   // (the watcher mask — subjects this node can probe, it has them as neighbours — is re-read where a watcher needs it: a handful of nodes)
-#define SFS_WMASK() ((busy & 4u) ? ((u32)p.watch[vl] >> p.sv_wshift) : 0u)   /* sv_wshift: the view a single-view launch works on (0 in every other launch) */
+#define SFS_WMASK() ((busy & BUSY_WATCH) ? ((u32)p.watch[vl] >> p.sv_wshift) : 0u)   /* sv_wshift: the view a single-view launch works on (0 in every other launch) */
   const bool ahead = !R1 && !STAGED && ah.valid;       // node word, peers' ids and the record of view pre.keep were requested a tile ago
   if (ahead) { ns = ah.ns; row0 = vl * p.udeg; row1 = row0 + p.udeg; }
   else if (!upfront) { load_node(); if (R1) load_rec0(); }
 
-  u32 clock = (u32)ns;
-  const bool up_r = (ns & NS_UP) != 0;
-  u32 sstate = (u32)(ns >> 40) & 3;
+  u32 clock = nw_clock(ns);
+  const bool up_r = nw_up(ns);
+  u32 sstate = nw_sstate(ns);
   const u32 deg = row1 - row0;
 
-  // host operation for this node (at most one per tick; the mark kernel set bit 1 of the busy byte)
+  // host operation for this node (at most one per tick)
   u32 op = 0, op_slot = 0;
-  if (busy & 2) { u32 slot_tmp = 0; op = cold_find_op(p, v, slot_tmp); op_slot = slot_tmp; }
+  if (busy & BUSY_OP) { u32 slot_tmp = 0; op = cold_find_op(p, v, slot_tmp); op_slot = slot_tmp; }
   bool up_s = up_r;
   if (op == OP_FAIL) up_s = false;
   if (op == OP_REJOIN) up_s = true;
@@ -585,13 +505,9 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   // SWIM probe target of this round (only matters while some tracked subject is down)
   bool have_probe = false;
   u32 ptarget = 0;
-  if (up_s && (busy & 4u) && p.probe_every && p.down_mask && ((t + v) % p.probe_every) == 0 && deg) {
+  if (up_s && (busy & BUSY_WATCH) && p.probe_every && p.down_mask && ((t + v) % p.probe_every) == 0 && deg) {
     ptarget = (STAGED && sv.col_staged) ? 0u : cold_probe_target(p, v, row0, deg);
-    if (STAGED && sv.col_staged) {
-      u32 w[4];
-      philox4x32_10(t, v, 0, DOMAIN_PROBE, p.seed_lo, p.seed_hi, w);
-      ptarget = sv.col[row0 + (((w[0] & 0xffffu) * deg) >> 16) - sv.col_base];
-    }
+    if (STAGED && sv.col_staged) ptarget = sv.col[row0 + neighbour_slot(t, v, DOMAIN_PROBE, p.seed_lo, p.seed_hi, deg) - sv.col_base];
     have_probe = true;
   }
 
@@ -605,7 +521,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   // Views to visit: all of them when the node as a whole has business (trace, reaper round, host operation, timers due);
   // otherwise those with mail, queued transmits or probe duty (a watcher's view of a subject that is down).
   const u32 all_views = (R >= 32u) ? 0xffffffffu : ((1u << R) - 1u);
-  const bool visit_all = R1 || TRACE || p.reap_now || (busy & 2u) || timers_due || !p.sleep_on;
+  const bool visit_all = R1 || TRACE || p.reap_now || (busy & BUSY_OP) || timers_due || !p.sleep_on;
   u32 todo = visit_all ? all_views : ((pre.mailmask | pre.qmask | (p.probe_every ? (SFS_WMASK() & p.down_mask) : 0u)) & all_views);
   if (!R1) SFS_COUNT(5, R - (u32)__popc(todo));             // views left asleep by a visited node
 
@@ -632,7 +548,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
     u32 q0;
     if (ahead && s == pre.keep) { cur = ah.rec; q0 = pre.qw; mL = pre.mL; mJ = pre.mJ; mM = pre.mM; SFS_PROBE(18); }
     else load_view(s, cur, q0, mL, mJ, mM);
-    merge_q(cur, q0);
+    merge_queue_word(cur, q0);
     first_view = s;
   }
 #pragma unroll 1
@@ -645,7 +561,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
     if (mM) st_u32_stream(p.inbox_rd + (size_t)(KIND_ML * R + s) * nl + vl, 0u, pol_first);
     const Words orig = cur;
     Rec r;
-    unpack_words(cur, r);
+    unpack(cur, r);
     const bool self = (p.subj[s] == v);
     const bool susp_before = up_r && r.mlstate == ML_SUSPECT;
     if (!R1 && p.sv_mode == SV_CHECK && !((sv_views >> s) & 1u) && up_r &&
@@ -654,18 +570,18 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
     // ---------------- Phase R ----------------
     if (up_r && (mL | mJ | mM)) {
       if (mM) {
-        const u32 key = mM - 1, inc = key >> 6, kind = (key >> 4) & 3, fromb = key & 15;
+        const u32 key = mM - 1, inc = ml_key_inc(key), kind = ml_key_state(key), fromb = ml_key_from(key);
         if (kind == ML_ALIVE) ml_alive(r, inc, self, limit);
         else if (kind == ML_SUSPECT) ml_suspect(r, inc, fromb, t, self, p.rules);
         else ml_dead(r, inc, kind == ML_LEFT, t, self, limit);
       }
       bool refute = false;
-      if (mL) { const u32 key = mL - 1, lt = key >> 1; witness(clock, lt); leave_intent(r, lt, !(key & 1u), self, sstate, refute, limit); }
+      if (mL) { const u32 key = mL - 1, lt = leave_key_lt(key); witness(clock, lt); leave_intent(r, lt, leave_key_prune(key), self, sstate, refute, limit); }
       if (mJ) { const u32 lt = mJ - 1; witness(clock, lt); join_intent(r, lt, limit); }
       if (refute) { Rec tr = r; u32 ck = clock; cold_refute(tr, ck, limit); r = tr; clock = ck; }
-      if (!(r.flags & 1) && r.status != TY_NONE && (r.status != (orig.w[6] & 0xff) || r.st != orig.w[0])) r.leave_tick = t + 1;   // NodeIntent.wall_time (types/member.rs:32)
+      stamp_intent(r, orig, t);
       Words mid;
-      pack_words(r, mid);
+      pack(r, mid);
       if (R1) c.cp += differs(mid, orig) ? 1u : 0u; else c.changed += differs(mid, orig) ? 1 : 0;
     }
     // ---------------- Phase E ----------------
@@ -680,11 +596,11 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
       const u32 mx = max(r.txl, max(r.txj, r.txm));
       if (mx) {
         if (!have_targets) {
-          if (ahead) nt = pick_finish<FMAX>(v, ah.cand, tg);
+          if (ahead) nt = peer_finish<FMAX>(v, ah.cand, tg);
           else {
             u32 cand[FMAX];
             pick_issue<FMAX, STAGED>(p, sv, v, row0, deg, pol_first, cand);
-            nt = pick_finish<FMAX>(v, cand, tg);
+            nt = peer_finish<FMAX>(v, cand, tg);
           }
           have_targets = true;
         }
@@ -714,35 +630,33 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
       if (self && sstate == SS_LEAVING && r.txl == 0 && r.mlstate == ML_ALIVE) {
         r.mlstate = ML_LEFT; r.qfrom = 0; r.txm = limit; sstate = SS_LEFT;
       }
-      // The trace's `pending` counts the views with queued transmits, a running suspicion timer, or a watcher that has not
-      // noticed yet.  Suspect views are counted by the persistent counter (they sleep), the others here.  A watcher's view of
-      // a down subject stays awake while it is Alive or Suspect: its own failed probe may still start or confirm the suspicion.
-      const bool queued = (r.txl | r.txj | r.txm) != 0;
-      if ((!R1 || PASS) && (queued || mx)) c.views |= 1u << (s + p.sv_slot * PASS);   // the view sent mail or keeps a queue: it has business in the next tick (passes, single-view ticks)
-      const bool watching = (busy & 4u) && p.probe_every && ((p.down_mask >> s) & 1) && !self && ((SFS_WMASK() >> s) & 1);
+      // Suspect views are counted in `pending` by the persistent counter (they sleep), the others here.
+      if ((!R1 || PASS) && (rec_queued(r) || mx)) c.views |= 1u << (s + p.sv_slot * PASS);   // the view sent mail or keeps a queue: it has business in the next tick (passes, single-view ticks)
+      // (view_watching / view_pending / view_awake of record.cuh, written out: through the helpers this kernel takes 32 more instructions)
+      const bool queued = rec_queued(r);
+      const bool watching = (busy & BUSY_WATCH) && p.probe_every && ((p.down_mask >> s) & 1) && !self && ((SFS_WMASK() >> s) & 1);
       const bool suspect = r.mlstate == ML_SUSPECT;
       { const u32 pnd = (!suspect && (queued || (watching && r.mlstate == ML_ALIVE))) ? 1u : 0u; if (R1) c.cp += pnd << 16; else c.pending += pnd; }
-      // (its own failed probe is a confirmation only while its bucket is not in the confirmer set and the set is not full)
       awake |= queued || (watching && (r.mlstate == ML_ALIVE || (suspect && cold_can_confirm(p.rules.k, r.mask, v))));
       if (suspect && r.deadline != 0) { has_timer = true; mind = min(mind, r.deadline); dl_moved |= r.deadline != orig.w[4]; }
     }
     dsusp += ((up_s && r.mlstate == ML_SUSPECT) ? 1 : 0) - (susp_before ? 1 : 0);
-    pack_words(r, cur);
+    pack(r, cur);
     {
       Words o2 = orig, c2 = cur;                           // storage image: record without budgets, budgets in the queue word
-      const u32 q_old = split_q(o2), q_new = split_q(c2);
+      const u32 q_old = split_queue_word(o2), q_new = split_queue_word(c2);
       if (differs(c2, o2)) st_rec256(p.rec + 2 * idx, c2, pol_first);
       if (q_new != q_old) { p.qword[idx] = q_new; SFS_COUNT(7, 4); }
     }
-    if (TRACE) c.hash += rec_hash((u64)s * p.n_global + v, make_uint4(cur.w[0], cur.w[1], cur.w[2], cur.w[3]), make_uint4(cur.w[4], cur.w[5], cur.w[6], cur.w[7]));
+    if (TRACE) c.hash += rec_hash((u64)s * p.n_global + v, cur);
     if (r.inc >= INC_LIMIT) *p.overflow = 1;
     if (!R1) {
       if (!SFS_VIEW_PREFETCH && s_next < R) load_view(s_next, nxt, nq, nL, nJ, nM);
-      cur = nxt; merge_q(cur, nq); mL = nL; mJ = nJ; mM = nM;
+      cur = nxt; merge_queue_word(cur, nq); mL = nL; mJ = nJ; mM = nM;
     }
     s = s_next;
   }
-  const u64 ns2 = (u64)clock | (up_s ? NS_UP : 0) | ((u64)sstate << 40);
+  const u64 ns2 = node_word(clock, up_s, sstate);
   if (ns2 != ns) st_u64_stream(p.node_state + vl, ns2, pol_first);
   if (TRACE) c.hash += node_hash((u64)R * p.n_global + v, ns2);
   if (clock >= LTIME_LIMIT) *p.overflow = 1;
@@ -755,13 +669,13 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   const bool exact = PASS ? (timers_due && !(cr & CARRY_SEEN)) : visit_all;
   // busy byte: the op bit is consumed, the watcher bit is static; the timer bit is exact after a visit of every view and
   // sticky otherwise (a view that was not visited may run a timer: it is found when its tile comes due)
-  const u32 busy2 = (awake_node ? 1u : 0u) | (busy & 4u) | ((has_timer || (!exact && (busy & 8u))) ? 8u : 0u);
+  const u32 busy2 = (awake_node ? BUSY_AWAKE : 0u) | (busy & BUSY_WATCH) | ((has_timer || (!exact && (busy & BUSY_TIMER))) ? BUSY_TIMER : 0u);
   if (busy2 != busy) p.busy[vl] = (u8)busy2;
   // node_due: a lower bound of the node's earliest running deadline, exact after a visit of every view.  A view's deadline only moves
   // while the view is visited, so views that were not visited are still covered by the word as it stands (in a pass: unless an earlier
   // pass rewrote the word exactly).
   if (has_timer) {
-    if (exact || !(busy & 8u)) p.node_due[vl] = mind;
+    if (exact || !(busy & BUSY_TIMER)) p.node_due[vl] = mind;
     else if (dl_moved || (PASS && (cr & CARRY_TDUE))) atomicMin(p.node_due + vl, mind);
   }
   if (PASS ? !timers_due : !visit_all) mind = min(mind, sleeping);   // its tile's entry was reset: timers of the views not visited go back with the node's word
@@ -799,8 +713,8 @@ template <bool TRACE>
 __device__ __forceinline__ void write_idle_row(const TickParams& p) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     SFS_PROBE(3);                                          // skipped ticks
-    p.row[4] += *reinterpret_cast<const u64*>(p.sched + SCHED_SUSPECTS);
-    if (TRACE && p.tick > 0) p.row[7] = *(p.row - 8 + 7);
+    p.row[ROW_PENDING] += *reinterpret_cast<const u64*>(p.sched + SCHED_SUSPECTS);
+    if (TRACE && p.tick > 0) p.row[ROW_HASH] = *(p.row - ROW_FIELDS + ROW_HASH);
   }
 }
 
@@ -836,8 +750,8 @@ __device__ __forceinline__ void publish_to_peer(u32 r, u32 world, u32 rank, u32 
   ctrl[me] = send_count[r];
   u64* sums = reinterpret_cast<u64*>(reinterpret_cast<unsigned char*>(peer_ctrl[r]) + CTRL_SUMS_OFF) + ((size_t)xpar * 8 + me) * CTRL_FIELDS;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) sums[i] = row[i];              // this rank's counters of the tick: every rank sums them on the device
-  sums[8] = sched[SCHED_LOCAL_QUIET]; sums[9] = sched[SCHED_LOCAL_UNTIL]; sums[10] = sched[SCHED_VIEWS_NEW];
+  for (int i = 0; i < ROW_FIELDS; ++i) sums[i] = row[i];              // this rank's counters of the tick: every rank sums them on the device
+  sums[ROW_FIELDS] = sched[SCHED_LOCAL_QUIET]; sums[ROW_FIELDS + 1] = sched[SCHED_LOCAL_UNTIL]; sums[ROW_FIELDS + 2] = sched[SCHED_VIEWS_NEW];
   __threadfence_system();
   st_release_sys(ctrl + 8 + me, stamp);
   send_count[r] = 0;
@@ -845,7 +759,7 @@ __device__ __forceinline__ void publish_to_peer(u32 r, u32 world, u32 rank, u32 
 
 // End of a tick: block reduction of the counters (warp shuffles, then shared memory) → one atomic per counter per CTA; the
 // LAST CTA to finish (ticket) completes the row and decides how long the cluster can sleep.
-// trace row: 0 packets, 1 edge_updates, 2 messages, 3 changed, 4 pending, (5 events, 6 suspects: direct), 7 hash
+// trace row: the first five fields (ROW_PACKETS .. ROW_PENDING) from the counters, (events, suspects: direct), hash
 template <bool TRACE, bool PACKED, bool PASS = false>
 __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters& c, u64 (*red)[BLOCK / 32], int dsusp_cta) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -867,14 +781,14 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
 #pragma unroll
     for (int w = 0; w < BLOCK / 32; ++w) s += red[threadIdx.x][w];
     if (s) {
-      if (threadIdx.x < 5) atomicAdd((unsigned long long*)(p.row + threadIdx.x), (unsigned long long)s);
+      if (threadIdx.x < ROW_EVENTS) atomicAdd((unsigned long long*)(p.row + threadIdx.x), (unsigned long long)s);
       else {
         atomicAdd(p.kinds_cur + (threadIdx.x - 5), (u32)min(s, (u64)0xffffffffu));
         if (PASS) atomicAdd(p.view_kinds_cur + (threadIdx.x - 5), (u32)min(s, (u64)0xffffffffu));   // a pass counts its own view only
       }
     }
   }
-  if (TRACE && lane == 0 && hs) atomicAdd((unsigned long long*)(p.row + 7), (unsigned long long)hs);
+  if (TRACE && lane == 0 && hs) atomicAdd((unsigned long long*)(p.row + ROW_HASH), (unsigned long long)hs);
   { const u32 vw = __reduce_or_sync(0xffffffffu, c.views); if (lane == 0 && vw) atomicOr(p.sched + SCHED_VIEWS_NEXT, vw); }
   if (PASS && p.sv_slot + 1u < p.sv_R) return;             // the last pass of the tick completes it
   // ---- ticket: every CTA's counters are in the row before the last one reads it ----
@@ -894,7 +808,7 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
   // (decided by ONE thread and broadcast: the words it reads are cleared below by thread 0, and a warp that evaluated them later than
   // thread 0 cleared them would take the other side of a branch that contains a barrier)
   __shared__ u32 quiet_s;
-  if (threadIdx.x == 0) quiet_s = (p.sleep_on && row[1] == 0 && row[2] == 0 && sched[SCHED_AWAKE] == 0 && sched[SCHED_UE_ACTIVITY] == 0) ? 1u : 0u;
+  if (threadIdx.x == 0) quiet_s = (p.sleep_on && row[ROW_EDGES] == 0 && row[ROW_MESSAGES] == 0 && sched[SCHED_AWAKE] == 0 && sched[SCHED_UE_ACTIVITY] == 0) ? 1u : 0u;
   __syncthreads();
   const bool quiet = quiet_s != 0;
   u32 until = p.tick + 1;
@@ -913,7 +827,7 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
     }
   }
   if (threadIdx.x == 0) {
-    row[4] = row[4] + suspects;                            // pending = awake views counted above + sleeping Suspect views
+    row[ROW_PENDING] = row[ROW_PENDING] + suspects;                            // pending = awake views counted above + sleeping Suspect views
     if (p.world == 1) {
       sched[SCHED_IDLE_UNTIL] = until;
       if (p.host_idle_until) *p.host_idle_until = until;
@@ -923,9 +837,9 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
     const u32 awake_n = sched[SCHED_AWAKE];
     sched[SCHED_AWAKE] = 0; sched[SCHED_UE_ACTIVITY] = 0; sched[SCHED_TICKET] = 0;
     // (the single-view kernel keeps no per-thread set: its view has business again iff anything was sent or anybody stays awake)
-    const u32 sv_next = (p.sv_mode == SV_SINGLE && (row[2] != 0 || awake_n != 0)) ? (1u << p.sv_slot) : 0u;
+    const u32 sv_next = (p.sv_mode == SV_SINGLE && (row[ROW_MESSAGES] != 0 || awake_n != 0)) ? (1u << p.sv_slot) : 0u;
     // this tick's set stays readable (OLD) for the kernel of this tick that is launched after this one and must return
-    const u32 sv_base = p.tick >= sched[SCHED_VIEWS_FROM] ? sched[SCHED_VIEWS_NEW] : sched[SCHED_VIEWS_OLD];   // what this kernel's CTAs read when they started (nobody else writes these words)
+    const u32 sv_base = views_of_tick(sched, p.tick);   // what this kernel's CTAs read when they started (nobody else writes these words)
     sched[SCHED_VIEWS_OLD] = sv_base; sched[SCHED_VIEWS_NEW] = sched[SCHED_VIEWS_NEXT] | sv_next; sched[SCHED_VIEWS_FROM] = p.tick + 1; sched[SCHED_VIEWS_NEXT] = 0;   // the views with business in the next tick (kernels that follow in this tick — anti-entropy, drain — add to it)
   }
   if (p.world > 1 && p.fuse_publish) {
@@ -954,16 +868,14 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   u32 sv_views = 0xffffffffu;
   bool work = true, carry_out = false;                     // PASS: this pass's view has business; so has a later pass's
   if (PASS) {
-    const u32 sv_base = p.tick >= p.sched[SCHED_VIEWS_FROM] ? p.sched[SCHED_VIEWS_NEW] : p.sched[SCHED_VIEWS_OLD];
-    const u32 views = (sv_base | p.views_host) & ((1u << p.sv_R) - 1u);
+    const u32 views = (views_of_tick(p.sched, p.tick) | p.views_host) & ((1u << p.sv_R) - 1u);
     work = (views >> p.sv_slot) & 1u;
     carry_out = (views >> p.sv_slot) > 1u;
     if (work) SFS_PROBE(21);
     else if (p.sv_slot != 0 && p.sv_slot + 1u < p.sv_R) return;    // neither node work nor a duty of the first or the last pass
   } else if (p.sv_mode != SV_OFF) {
     // (the kernel of this tick that ran before this one, if any, has already published the NEXT tick's set: SCHED_VIEWS_FROM says since when it holds)
-    const u32 sv_base = p.tick >= p.sched[SCHED_VIEWS_FROM] ? p.sched[SCHED_VIEWS_NEW] : p.sched[SCHED_VIEWS_OLD];
-    const u32 views = (sv_base | p.views_host) & ((1u << p.sv_R) - 1u);
+    const u32 views = (views_of_tick(p.sched, p.tick) | p.views_host) & ((1u << p.sv_R) - 1u);
     const bool single = views == (1u << p.sv_slot);        // exactly the one view the single-view launch was set up for
     if (p.sv_mode == SV_SINGLE) { if (!single) return; SFS_PROBE(21); }
     else if (p.sv_mode == SV_GENERAL && single) return;
@@ -981,15 +893,12 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
   bool wrote_remote = false;
   u32 resv = 0, rlen = 0;                                  // lane s: the entries this warp holds reserved in peer s's window (flush_xwarp)
 
-  // Dense / sparse ticks.  While the gossip front is wide (the previous tick sent at least one message per
-  // two tiles) every tile will be hot anyway: senders skip the per-message tile marking and the next tick
-  // simply processes everything (kinds[3] of this tick's row records the decision).  In sparse ticks each
-  // delivery marks its destination tile, and tiles nobody touched are not read at all.
-  const u32 prev_msgs = p.kinds_prev[KIND_LEAVE] + p.kinds_prev[KIND_JOIN] + p.kinds_prev[KIND_ML];
-  const bool dense_now = prev_msgs >= (p.n_tiles >> 1) + 1;      // what this tick's sends will look like
+  // Dense / sparse ticks (dense_tick, tick_kernel.cuh): kinds[3] of this tick's counters records the decision.
+  const u32 prev_msgs = sent_messages(p.kinds_prev);
+  const bool dense_now = dense_tick(prev_msgs, p.n_tiles);       // what this tick's sends will look like
   const bool all_hot = p.force_all || p.kinds_prev[3] != 0;      // the previous tick was dense (or skipping is off)
   const bool mark = !dense_now;
-  const u32 own_msgs = PASS ? kv[KIND_LEAVE] + kv[KIND_JOIN] + kv[KIND_ML] : prev_msgs;
+  const u32 own_msgs = PASS ? sent_messages(kv) : prev_msgs;
   const bool saturated = own_msgs >= (p.n_local >> 1);           // most nodes have mail: request record + node word up front
   if (dense_now && blockIdx.x == 0 && threadIdx.x == 0) p.kinds_cur[3] = 1;
   if (PASS && work && threadIdx.x == 0) {                        // coverage of the host build: decisions the whole-tick counters would have taken otherwise
@@ -1038,12 +947,12 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
       for (u32 g = 0; g < GROUP; ++g) {
         const bool due_g = g < ng && (hot_s[gt_s[g]] & 2u) != 0;
         Pre prg = pr[g];
-        if (due_g && (prg.busy & 8u)) prg.nd = p.node_due[((tile0 + gt_s[g]) << TILE_SHIFT) + threadIdx.x];
+        if (due_g && (prg.busy & BUSY_TIMER)) prg.nd = p.node_due[((tile0 + gt_s[g]) << TILE_SHIFT) + threadIdx.x];
         const bool act = g < ng && node_active<PASS>(p, prg, due_g);   // lanes past n_local hold an empty Pre
         if (due_g) {                                         // (warp-uniform) nodes whose own timers run later hand their deadline back to the wheel
           const u32 wm = warp_min(act ? NO_DEADLINE : sleeping_deadline(prg, true));
           if (lane == 0 && wm != NO_DEADLINE) atomicMin(p.tile_due + tile0 + gt_s[g], wm);
-          if (!act && (prg.busy & 8u)) SFS_PROBE(20);
+          if (!act && (prg.busy & BUSY_TIMER)) SFS_PROBE(20);
         }
         const u32 bal = __ballot_sync(0xffffffffu, act);
         if (bal) {
@@ -1162,8 +1071,7 @@ __global__ void __launch_bounds__(BLOCK, 3) tick_kernel_tma(const __grid_constan
   const u64 pol_first = policy_evict_first(), pol_last = policy_evict_last();
   const int lane = threadIdx.x & 31;
 
-  const u32 prev_msgs = p.kinds_prev[KIND_LEAVE] + p.kinds_prev[KIND_JOIN] + p.kinds_prev[KIND_ML];
-  const bool dense_now = prev_msgs >= (p.n_tiles >> 1) + 1;
+  const bool dense_now = dense_tick(sent_messages(p.kinds_prev), p.n_tiles);
   const bool all_hot = p.force_all || p.kinds_prev[3] != 0;
   const bool mark = !dense_now;
   if (dense_now && blockIdx.x == 0 && threadIdx.x == 0) p.kinds_cur[3] = 1;
@@ -1267,12 +1175,10 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
   for (u32 vl = blockIdx.x * BLOCK + threadIdx.x; vl < p.n_local; vl += gridDim.x * BLOCK) {
     const u32 v = p.first + vl;
     const u64 ns = snap_node[vl];
-    if (!(ns & NS_UP)) continue;
+    if (!nw_up(ns)) continue;
     const u32 row0 = p.row_ptr[vl], deg = p.row_ptr[vl + 1] - row0;
     if (!deg) continue;
-    u32 w[4];
-    philox4x32_10(p.tick, v, 0, DOMAIN_PUSHPULL, p.seed_lo, p.seed_hi, w);
-    const u32 u = p.col[row0 + (((w[0] & 0xffffu) * deg) >> 16)];
+    const u32 u = p.col[row0 + neighbour_slot(p.tick, v, DOMAIN_PUSHPULL, p.seed_lo, p.seed_hi, deg)];
     if (u == v) continue;
     // the partner may live in another shard: its rank's snapshot is read through the peer mapping (the host
     // separates "every rank has taken its snapshot" and "every rank has finished reading" with barriers)
@@ -1284,29 +1190,28 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
       const u32 shard = u / p.shard_size;
       ul = u - shard * p.shard_size;
       part_node = p.snap_node_peer[shard]; part_rec = p.snap_rec_peer[shard];
-      const u32 cnt = min(p.shard_size, p.n_global - shard * p.shard_size);
-      part_stride = ((cnt + BLOCK - 1) / BLOCK) * BLOCK;
+      part_stride = plane_stride(min(p.shard_size, p.n_global - shard * p.shard_size));
     }
     const u64 nu = part_node[ul];
-    if (!(nu & NS_UP)) continue;
-    u32 clock = (u32)ns;
-    const u32 sstate = (u32)(ns >> 40) & 3;
-    const u32 cu = (u32)nu;
+    if (!nw_up(nu)) continue;
+    u32 clock = nw_clock(ns);
+    const u32 sstate = nw_sstate(ns);
+    const u32 cu = nw_clock(nu);
     if (cu > 0) witness(clock, cu - 1);
     bool awake = false, has_timer = false;
     u32 mind = NO_DEADLINE;
     const u32 wmask = p.watch[vl];
     for (u32 s = 0; s < p.R; ++s) {
       const size_t iv = (size_t)s * p.stride + vl, iu = (size_t)s * part_stride + ul;
-      const uint4 a0 = p.rec[2 * iv];
-      uint4 b0 = p.rec[2 * iv + 1];
+      Words w0 = load_rec(p.rec, iv);
       const u32 q0 = p.qword[iv];
-      merge_queue_word(b0, q0);
+      merge_queue_word(w0, q0);
       Rec r, q;
-      unpack(a0, b0, r);
-      unpack(part_rec[2 * iu], part_rec[2 * iu + 1], q);
+      unpack(w0, r);
+      unpack(load_rec(part_rec, iu), q);
       const bool self = (p.subj[s] == v);
-      const bool was = (r.txl | r.txj | r.txm) || r.mlstate == ML_SUSPECT || (p.probe_every && ((p.down_mask >> s) & 1) && !self && ((wmask >> s) & 1) && r.mlstate == ML_ALIVE);
+      const bool watching = view_watching(wmask != 0, p.probe_every, p.down_mask, s, self, wmask);
+      const bool was = view_pending(r, watching) || r.mlstate == ML_SUSPECT;
       if (q.flags & 1) {
         if (q.mlstate == ML_ALIVE) ml_alive(r, q.inc, self, p.rules.limit);
         else if (q.mlstate == ML_LEFT) ml_dead(r, q.inc, true, p.tick, self, p.rules.limit);
@@ -1314,28 +1219,27 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
         bool refute = false;
         if (q.status == ST_LEFT) { witness(clock, q.st + 1); leave_intent(r, q.st + 1, false, self, sstate, refute, p.rules.limit, false); }
         else { witness(clock, q.st); join_intent(r, q.st, p.rules.limit, false); }
-        if (refute) { const u32 T = clock; witness(clock, T); join_intent(r, T, p.rules.limit); r.qjoin = T; r.txj = p.rules.limit; }
-        if (!(r.flags & 1) && r.status != TY_NONE && (r.status != (b0.z & 0xff) || r.st != a0.x)) r.leave_tick = p.tick + 1;
+        if (refute) refute_leave(r, clock, p.rules.limit);
+        stamp_intent(r, w0, p.tick);
       }
-      uint4 a1, b1;
-      pack(r, a1, b1);
-      const bool ch = (a1.x ^ a0.x) | (a1.y ^ a0.y) | (a1.z ^ a0.z) | (a1.w ^ a0.w) | (b1.x ^ b0.x) | (b1.y ^ b0.y) | (b1.z ^ b0.z) | (b1.w ^ b0.w);
+      Words w1;
+      pack(r, w1);
+      const bool ch = differs(w1, w0);
       if (ch) {
-        uint4 bs = b1;
-        const u32 q1 = split_queue_word(bs);
-        p.rec[2 * iv] = a1; p.rec[2 * iv + 1] = bs;
+        Words ws = w1;
+        const u32 q1 = split_queue_word(ws);
+        store_rec(p.rec, iv, ws);
         if (q1 != q0) p.qword[iv] = q1;
       }
-      if ((a1.y ^ a0.y) | (a1.z ^ a0.z) | (a1.w ^ a0.w) | (b1.x ^ b0.x) | (b1.y ^ b0.y) | (b1.z ^ b0.z) | (b1.w ^ b0.w)) { d_changed++; SFS_PROBE(28); }   // status_time creep is not a change
-      if (TRACE && ch) d_hash += rec_hash((u64)s * p.n_global + v, a1, b1) - rec_hash((u64)s * p.n_global + v, a0, b0);
-      const bool watching = p.probe_every && ((p.down_mask >> s) & 1) && !self && ((wmask >> s) & 1);
-      const bool now = (r.txl | r.txj | r.txm) || r.mlstate == ML_SUSPECT || (watching && r.mlstate == ML_ALIVE);
-      d_pending += (now ? 1 : 0) - (was ? 1 : 0);
-      d_susp += (r.mlstate == ML_SUSPECT ? 1 : 0) - (((b0.z >> 8) & 3u) == ML_SUSPECT ? 1 : 0);     // the node is up: counted views
-      awake |= (r.txl | r.txj | r.txm) != 0 || (watching && (r.mlstate == ML_ALIVE ||
-               (r.mlstate == ML_SUSPECT && (u32)__popc(r.mask) - 1u < p.rules.k && !(r.mask & (1u << from_bucket(v))))));
+      Words wt = w1;                                       // status_time creep is not a change
+      wt.w[0] = w0.w[0];
+      if (differs(wt, w0)) { d_changed++; SFS_PROBE(28); }
+      if (TRACE && ch) d_hash += rec_hash((u64)s * p.n_global + v, w1) - rec_hash((u64)s * p.n_global + v, w0);
+      d_pending += (view_pending(r, watching) || r.mlstate == ML_SUSPECT ? 1 : 0) - (was ? 1 : 0);
+      d_susp += (r.mlstate == ML_SUSPECT ? 1 : 0) - (((w0.w[6] >> 8) & 3u) == ML_SUSPECT ? 1 : 0);     // the node is up: counted views
+      awake |= view_awake(r, watching, [&] { return can_confirm(p.rules.k, r.mask, v); });
       if (r.mlstate == ML_SUSPECT && r.deadline != 0) { has_timer = true; mind = min(mind, r.deadline); }
-      if (r.txl | r.txj | r.txm) d_views |= 1u << s;
+      if (rec_queued(r)) d_views |= 1u << s;
       if (r.inc >= INC_LIMIT) *p.overflow = 1;
     }
     if (p.ue_table.n) {                                        // the partner's event clock and ring (a snapshot, like its records)
@@ -1354,14 +1258,14 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
       if (TRACE) d_hash += ue_hash((u64)(p.R + 1) * p.n_global + v, w1) - ue_hash((u64)(p.R + 1) * p.n_global + v, w0);
       if (er.clock >= LTIME_LIMIT) *p.overflow = 1;
     }
-    const u64 ns2 = (ns & ~0xffffffffull) | clock;
+    const u64 ns2 = node_word(clock, nw_up(ns), sstate);
     if (ns2 != ns) {
       p.node_state[vl] = ns2;
       if (TRACE) d_hash += node_hash((u64)p.R * p.n_global + v, ns2) - node_hash((u64)p.R * p.n_global + v, ns);
     }
     if (clock >= LTIME_LIMIT) *p.overflow = 1;
-    // every view of the node was visited: its busy byte is exact (bit 0 awake, bit 2 watcher, bit 3 running timer)
-    p.busy[vl] = (u8)((awake ? 1u : 0u) | (wmask ? 4u : 0u) | (has_timer ? 8u : 0u));
+    // every view of the node was visited: its busy byte is exact
+    p.busy[vl] = (u8)((awake ? BUSY_AWAKE : 0u) | (wmask ? BUSY_WATCH : 0u) | (has_timer ? BUSY_TIMER : 0u));
     if (awake) p.hot_wr[vl >> TILE_SHIFT] = 1;
     if (has_timer) { atomicMin(p.tile_due + (vl >> TILE_SHIFT), mind); p.node_due[vl] = mind; }
   }
@@ -1369,10 +1273,10 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
   d_views = __reduce_or_sync(0xffffffffu, d_views);
   if ((threadIdx.x & 31) == 0) {
     if (d_views) atomicOr(p.sched + SCHED_VIEWS_NEW, d_views);
-    if (c) atomicAdd((unsigned long long*)(p.row + 3), (unsigned long long)c);
-    if (q) atomicAdd((unsigned long long*)(p.row + 4), (unsigned long long)q);
+    if (c) atomicAdd((unsigned long long*)(p.row + ROW_CHANGED), (unsigned long long)c);
+    if (q) atomicAdd((unsigned long long*)(p.row + ROW_PENDING), (unsigned long long)q);
     if (ds) atomicAdd(reinterpret_cast<unsigned long long*>(p.sched + SCHED_SUSPECTS), (unsigned long long)ds);
-    if (TRACE && h) atomicAdd((unsigned long long*)(p.row + 7), (unsigned long long)h);
+    if (TRACE && h) atomicAdd((unsigned long long*)(p.row + ROW_HASH), (unsigned long long)h);
   }
 }
 
@@ -1394,7 +1298,7 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
   }
   __syncthreads();
   // global trace row of this tick: my counters + the rows the peers published with their flags (acquired above)
-  if (blockIdx.x == 0 && threadIdx.x < 8) {
+  if (blockIdx.x == 0 && threadIdx.x < ROW_FIELDS) {
     u64 s = p.my_row[threadIdx.x];
     for (u32 src = 0; src < p.world; ++src) if (src != p.rank) s += __ldcg(p.sums + (size_t)src * CTRL_FIELDS + threadIdx.x);
     p.grow[threadIdx.x] = s;
@@ -1408,18 +1312,17 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
     u32 until = p.sched[SCHED_LOCAL_UNTIL];
     for (u32 src = 0; src < p.world; ++src) {
       if (src == p.rank) continue;
-      quiet = quiet && __ldcg(p.sums + (size_t)src * CTRL_FIELDS + 8) != 0;
-      until = min(until, (u32)__ldcg(p.sums + (size_t)src * CTRL_FIELDS + 9));
+      quiet = quiet && __ldcg(p.sums + (size_t)src * CTRL_FIELDS + ROW_FIELDS) != 0;
+      until = min(until, (u32)__ldcg(p.sums + (size_t)src * CTRL_FIELDS + ROW_FIELDS + 1));
     }
     if (p.host_idle_until) *p.host_idle_until = quiet ? max(until, p.tick + 1) : p.tick + 1;
     u32 views = 0;                                        // views with business in the next tick: anywhere in the cluster (their mail crosses shards)
-    for (u32 src = 0; src < p.world; ++src) if (src != p.rank) views |= (u32)__ldcg(p.sums + (size_t)src * CTRL_FIELDS + 10);
+    for (u32 src = 0; src < p.world; ++src) if (src != p.rank) views |= (u32)__ldcg(p.sums + (size_t)src * CTRL_FIELDS + ROW_FIELDS + 2);
     if (views) atomicOr(p.sched_rw + SCHED_VIEWS_NEW, views);
   }
-  // same dense / sparse decision as the tick kernel of this tick: in a dense tick the next tick processes every
+  // the tick kernel's dense / sparse decision of this tick: in a dense tick the next tick processes every
   // tile anyway, so per-entry tile marking (millions of byte stores onto a few thousand flags) is skipped
-  const u32 prev_msgs = p.kinds_prev[KIND_LEAVE] + p.kinds_prev[KIND_JOIN] + p.kinds_prev[KIND_ML];
-  const bool mark = prev_msgs < (p.n_tiles >> 1) + 1;
+  const bool mark = !dense_tick(sent_messages(p.kinds_prev), p.n_tiles);
   u32 seen = 0;                                 // kinds this thread folded (bit per kind)
   for (u32 src = 0; src < p.world; ++src) {
     if (src == p.rank) continue;
@@ -1430,28 +1333,27 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
       if (e == 0) continue;                          // padding of a partly filled block (a real entry has value + 1 > 0 in its high word)
       if (!p.byz_on) w[i] = 0;                       // consumed: the window reads as zeros when it is written next (injector triples are
                                                      // read by a neighbouring thread too: those runs clear the windows in a kernel of their own)
-      const u32 val1 = (u32)(e >> 32), s = (u32)(e >> 28) & 15, kind = (u32)(e >> 26) & 3;
-      u32 dl = (u32)e & ((1u << 26) - 1);
+      const u32 val1 = win_val1(e), s = win_slot(e), kind = win_kind(e);
+      u32 dl = win_dst(e);
       const bool byz = p.byz_on && (dl & BYZ_FLAG);
       if (byz) dl &= ~BYZ_FLAG;
-      if (byz && kind == 3 && s == BYZ_ANNOT_SLOT) continue;           // third entry of a triple: read by the thread holding the first
+      if (byz && kind == KIND_EXTRA && s == BYZ_ANNOT_SLOT) continue;           // third entry of a triple: read by the thread holding the first
       if (dl < p.n_local && s < p.R && kind < 3) {
         atomicMax(p.inbox_wr + ((size_t)(kind * p.R + s)) * p.stride + dl, val1);
         if (mark) p.hot_wr[dl >> TILE_SHIFT] = 1;
         seen |= 1u << kind;
         if (byz && kind < 2 && i + 2 < n) {                            // first entry of a triple: judge it against MY record, flag the sender in ITS shard
           const u64 e1 = __ldcg(w + i + 1), e2 = __ldcg(w + i + 2);
-          const u32 src = (u32)(e2 >> 32) - 1u;
+          const u32 src = win_val1(e2) - 1u;
           ByzEntries be{};
-          be.serf_lt = kind == KIND_LEAVE ? (val1 - 1u) >> 1 : val1 - 1u; be.ml_inc = ((u32)(e1 >> 32) - 1u) >> 6;
-          if (p.node_state[dl] & NS_UP) {
-            const size_t iv = (size_t)s * p.stride + dl;
+          be.serf_lt = kind == KIND_LEAVE ? leave_key_lt(val1 - 1u) : val1 - 1u; be.ml_inc = ml_key_inc(win_val1(e1) - 1u);
+          if (nw_up(p.node_state[dl])) {
             Rec q;
-            unpack(p.rec[2 * iv], p.rec[2 * iv + 1], q);
+            unpack(load_rec(p.rec, (size_t)s * p.stride + dl), q);
             if (byz_anomalous(q, be, p.byz_delta)) { const u32 sh = src / p.shard_size; p.peer_anomaly[sh][src - sh * p.shard_size] = 1; }
           }
         }
-      } else if (dl < p.n_local && kind == 3 && s < p.ue_n && val1) {   // user event s arrived: one bit, and the time its origin stamped
+      } else if (dl < p.n_local && kind == KIND_EXTRA && s < p.ue_n && val1) {   // user event s arrived: one bit, and the time its origin stamped
         atomicOr(p.ue_inbox_wr + dl, 1u << s);
         p.ue_ltime[s] = val1 - 1;                      // every copy carries the same value; this shard learns it no later than the event itself
       }
@@ -1470,11 +1372,13 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
 __global__ void fill_idle_rows_kernel(u64* rows, u64* grow_rows, u32 n, const u32* sched, int trace) {
   const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  rows[(size_t)i * 8 + 4] = *reinterpret_cast<const u64*>(sched + SCHED_SUSPECTS);
-  if (trace) rows[(size_t)i * 8 + 7] = *(rows - 8 + 7);
+  u64* const row = rows + (size_t)i * ROW_FIELDS;
+  row[ROW_PENDING] = *reinterpret_cast<const u64*>(sched + SCHED_SUSPECTS);
+  if (trace) row[ROW_HASH] = *(rows - ROW_FIELDS + ROW_HASH);
   if (grow_rows) {                                         // sharded: the global rows repeat the global pending count / hash
-    grow_rows[(size_t)i * 8 + 4] = *(grow_rows - 8 + 4);
-    if (trace) grow_rows[(size_t)i * 8 + 7] = *(grow_rows - 8 + 7);
+    u64* const grow = grow_rows + (size_t)i * ROW_FIELDS;
+    grow[ROW_PENDING] = *(grow_rows - ROW_FIELDS + ROW_PENDING);
+    if (trace) grow[ROW_HASH] = *(grow_rows - ROW_FIELDS + ROW_HASH);
   }
 }
 
@@ -1506,7 +1410,7 @@ __global__ void compute_watch_kernel(const u32* __restrict__ row_ptr, const u32*
 __global__ void apply_watch_kernel(const u16* __restrict__ watch, u32 n_local, u8* busy, u8* hot_static) {
   const u32 vl = blockIdx.x * blockDim.x + threadIdx.x;
   if (vl >= n_local || watch[vl] == 0) return;
-  busy[vl] |= 4;
+  busy[vl] |= BUSY_WATCH;
   hot_static[vl >> TILE_SHIFT] = 1;              // a watcher's tile is scheduled every tick (static flags: never consumed)
 }
 
@@ -1515,13 +1419,10 @@ __global__ void init_state_kernel(uint4* rec, u64* node_state, u32 n_local, u32 
   if (vl >= n_local) return;
   Rec r = {};
   r.st = init_st; r.inc = 1; r.status = ST_ALIVE; r.mlstate = ML_ALIVE; r.flags = 1;
-  uint4 a, b;
-  pack(r, a, b);
-  for (u32 s = 0; s < R; ++s) {
-    const size_t idx = (size_t)s * stride + vl;
-    rec[2 * idx] = a; rec[2 * idx + 1] = b;
-  }
-  node_state[vl] = (u64)init_clock | NS_UP;
+  Words x;
+  pack(r, x);
+  for (u32 s = 0; s < R; ++s) store_rec(rec, (size_t)s * stride + vl, x);
+  node_state[vl] = node_word(init_clock, true, SS_ALIVE);
 }
 
 __global__ void mark_events_kernel(u8* busy, u8* hot_rd, const u32* ev_node, u32 ev_begin, u32 ev_end, u32 first, u32 n_local) {
@@ -1529,7 +1430,7 @@ __global__ void mark_events_kernel(u8* busy, u8* hot_rd, const u32* ev_node, u32
   if (e >= ev_end) return;
   const u32 vl = ev_node[e] - first;
   if (vl < n_local) {
-    busy[vl] |= 2;                                 // one op per (node, tick): no two threads touch the same byte
+    busy[vl] |= BUSY_OP;                           // one op per (node, tick): no two threads touch the same byte
     hot_rd[vl >> TILE_SHIFT] = 1;                  // the tile must run this tick
   }
 }
@@ -1537,11 +1438,10 @@ __global__ void mark_events_kernel(u8* busy, u8* hot_rd, const u32* ev_node, u32
 __global__ void extract_kernel(const uint4* rec, const u64* node_state, u32 n_local, u32 stride, u32 slot, int what, void* out) {
   const u32 vl = blockIdx.x * blockDim.x + threadIdx.x;
   if (vl >= n_local) return;
-  if (what == EXTRACT_CLOCK) { ((u64*)out)[vl] = node_state[vl] & 0xffffffffull; return; }
-  if (what == EXTRACT_CLOCK32) { ((u32*)out)[vl] = (u32)node_state[vl]; return; }
-  const size_t idx = (size_t)slot * stride + vl;
+  if (what == EXTRACT_CLOCK) { ((u64*)out)[vl] = nw_clock(node_state[vl]); return; }
+  if (what == EXTRACT_CLOCK32) { ((u32*)out)[vl] = nw_clock(node_state[vl]); return; }
   Rec r;
-  unpack(rec[2 * idx], rec[2 * idx + 1], r);
+  unpack(load_rec(rec, (size_t)slot * stride + vl), r);
   const bool known = r.flags & 1;
   switch (what) {
     case EXTRACT_STATUS: ((u8*)out)[vl] = known ? (u8)r.status : (u8)ST_NONE; break;
@@ -1556,9 +1456,9 @@ __global__ void compose_records_kernel(const uint4* rec, const u32* qword, u32 n
   const u32 vl = blockIdx.x * blockDim.x + threadIdx.x;
   if (vl >= n_local) return;
   const size_t idx = (size_t)slot * stride + vl;
-  uint4 b = rec[2 * idx + 1];
-  merge_queue_word(b, qword[idx]);
-  out[2 * (size_t)vl] = rec[2 * idx]; out[2 * (size_t)vl + 1] = b;
+  Words x = load_rec(rec, idx);
+  merge_queue_word(x, qword[idx]);
+  store_rec(out, vl, x);
 }
 
 __global__ void __launch_bounds__(BLOCK) state_hash_kernel(const uint4* rec, const u32* qword, const u64* node_state, u32 n_local, u32 stride, u32 first, u32 n_global, u32 R, u64* out) {
@@ -1566,9 +1466,9 @@ __global__ void __launch_bounds__(BLOCK) state_hash_kernel(const uint4* rec, con
   for (u32 vl = blockIdx.x * BLOCK + threadIdx.x; vl < n_local; vl += gridDim.x * BLOCK) {
     for (u32 s = 0; s < R; ++s) {
       const size_t idx = (size_t)s * stride + vl;
-      uint4 b = rec[2 * idx + 1];
-      merge_queue_word(b, qword[idx]);
-      h += rec_hash((u64)s * n_global + first + vl, rec[2 * idx], b);
+      Words x = load_rec(rec, idx);
+      merge_queue_word(x, qword[idx]);
+      h += rec_hash((u64)s * n_global + first + vl, x);
     }
     h += node_hash((u64)R * n_global + first + vl, node_state[vl]);
   }
@@ -1585,12 +1485,12 @@ __global__ void __launch_bounds__(BLOCK) summary_kernel(const uint4* rec, const 
     const u32 sid = subj[s];
     for (u32 vl = blockIdx.x * BLOCK + threadIdx.x; vl < n_local; vl += gridDim.x * BLOCK) {
       const u64 ns = node_state[vl];
-      if (s == 0) maxclock = max(maxclock, (u64)(ns & 0xffffffffull));
+      if (s == 0) maxclock = max(maxclock, (u64)nw_clock(ns));
       const size_t idx = (size_t)s * stride + vl;
       Rec r;
-      unpack(rec[2 * idx], rec[2 * idx + 1], r);
+      unpack(load_rec(rec, idx), r);
       { const u32 q = qword[idx]; queued += ((q & 0xffu) ? 1 : 0) + (((q >> 8) & 0xffu) ? 1 : 0); }
-      if ((ns & NS_UP) && sid != first + vl) {
+      if (nw_up(ns) && sid != first + vl) {
         const bool known = r.flags & 1;
         const u64 key = (((u64)r.st << 32) ^ ((u64)r.inc << 8) ^ ((u64)(known ? r.status : 0) << 4) ^ r.mlstate ^ ((u64)known << 63));
         kmin = min(kmin, key); kmax = max(kmax, key);
@@ -1621,7 +1521,7 @@ int tick_ctas_per_sm_r1() { return SFS_MB_R1; }
 int tick_ctas_per_sm_r1s() { return SFS_MB_R1S; }
 int tick_ctas_per_sm_rn() { return SFS_MB_RN; }
 int tick_grid_size(u32 n_local, int ctas_per_sm, int sms, int gridmul) {
-  const u32 tiles = (n_local + BLOCK - 1) / BLOCK;
+  const u32 tiles = plane_stride(n_local) >> TILE_SHIFT;
   u32 grid = (u32)sms * (u32)ctas_per_sm * (u32)gridmul;    // persistent: SM count × resident CTAs × 2 (two waves for balance)
   if (tiles < grid) grid = tiles ? tiles : 1;
   while ((tiles + grid - 1) / grid > MAX_TILES_PER_CTA) grid += (u32)sms * (u32)ctas_per_sm;
@@ -1668,14 +1568,8 @@ void launch_tick_pass(const TickParams& p, int grid, cudaStream_t st) {
 }
 // The single-view kernel of a dual launch of a sharded run (SV_SINGLE): the single-slot kernel on the one view that has business (multi-slot plane layout).
 void launch_tick_single_view(const TickParams& p, int grid, cudaStream_t st) {
-  const bool sharded = p.world > 1;
-  if (p.fanout <= 4) {
-    if (sharded) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 4, true, true, SFS_MB_R1S>)(p);
-    else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 4, false, true, SFS_MB_R1>)(p);
-  } else {
-    if (sharded) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 8, true, true, SFS_MB_R1S>)(p);
-    else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 8, false, true, SFS_MB_R1>)(p);
-  }
+  if (p.fanout <= 4) SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 4, true, true, SFS_MB_R1S>)(p);
+  else SFS_LAUNCH(grid, BLOCK, 0, st, tick_kernel<false, 8, true, true, SFS_MB_R1S>)(p);
 }
 void launch_fill_idle_rows(u64* rows, u64* grow_rows, u32 n, const u32* sched, bool trace, cudaStream_t st) {
   if (n) SFS_LAUNCH((n + 127) / 128, 128, 0, st, fill_idle_rows_kernel)(rows, grow_rows, n, sched, trace ? 1 : 0);

@@ -27,6 +27,44 @@ constexpr int SFS_SMS = 1;
 
 namespace sfs {
 
+constexpr u32 TILE_SHIFT = 8, TILE = 1u << TILE_SHIFT;   // one tile = one CTA pass of the tick kernels = 256 nodes
+// Per-slot planes hold a whole number of tiles: the stride of a plane in nodes.
+SFS_HD u32 plane_stride(u32 n) { return ((n + TILE - 1) >> TILE_SHIFT) << TILE_SHIFT; }
+
+// Trace row of a tick (serfsim_tick_row_t, static_asserts in serfsim.cu): ROW_FIELDS u64 counters
+enum : u32 { ROW_PACKETS = 0, ROW_EDGES = 1, ROW_MESSAGES = 2, ROW_CHANGED = 3, ROW_PENDING = 4, ROW_EVENTS = 5, ROW_SUSPECTS = 6, ROW_HASH = 7, ROW_FIELDS = 8 };
+
+// Dense / sparse ticks.  While the gossip front is wide (the previous tick sent at least one message per two tiles) every
+// tile will be hot anyway: senders skip the per-message tile marking and the next tick simply processes everything.  In
+// sparse ticks each delivery marks its destination tile, and tiles nobody touched are not read at all.
+SFS_HD u32 sent_messages(const u32* kinds) { return kinds[KIND_LEAVE] + kinds[KIND_JOIN] + kinds[KIND_ML]; }
+SFS_HD bool dense_tick(u32 prev_msgs, u32 n_tiles) { return prev_msgs >= (n_tiles >> 1) + 1; }
+
+// Cross-shard window entry (8 B): value + 1 << 32 | view << 28 | kind << 26 | destination (26 bits, local to its shard).
+// Kind 3 (KIND_EXTRA) is a user event (view = the event) or the annotation of an injector triple (ByzParams).
+constexpr u32 KIND_EXTRA = 3;
+SFS_HD u64 win_entry(u32 val1, u32 s, u32 kind, u32 dloc) { return ((u64)val1 << 32) | ((u64)s << 28) | ((u64)kind << 26) | dloc; }
+SFS_HD u32 win_val1(u64 e) { return (u32)(e >> 32); }
+SFS_HD u32 win_slot(u64 e) { return (u32)(e >> 28) & 15; }
+SFS_HD u32 win_kind(u64 e) { return (u32)(e >> 26) & 3; }
+SFS_HD u32 win_dst(u64 e) { return (u32)e & ((1u << 26) - 1); }
+// Append N entries to this rank's segment of peer `shard`'s window (P: a parameter block with the window fields); a full
+// window raises overflow 2.
+template <u32 N, class P>
+__device__ __forceinline__ void win_append(const P& p, u32 shard, const u64 (&e)[N]) {
+  const u32 g = atomicAdd(p.send_count + shard, N);
+  if (g + (N - 1) < p.win_cap) {
+#pragma unroll
+    for (u32 i = 0; i < N; ++i) p.win_data[shard][(size_t)p.rank * p.win_cap + g + i] = e[i];
+  } else {
+    *p.overflow = 2;
+  }
+}
+
+// Cross-shard staging of the tick kernel: staged entries per warp (3 KB), split evenly over the world-1 peers (world 8: 56 each)
+// (TickParams::xcap); a full warp-wide store flushes; at most XW_RESERVE_MAX entries reserved ahead per warp and peer.
+constexpr u32 XW_TOTAL = 392, XW_FLUSH = 32, XW_RESERVE_MAX = 128;
+
 // Device-side convergence gate (serfsim_run_until_converged).  The host launches ticks in large chunks without looking at
 // their rows; the FIRST kernel of tick t evaluates the quiescence rule on the (global) row of tick t-1 and, when the run is
 // over, sets a sticky word — that kernel and every later kernel of the call then return at once, so ticks launched past the
@@ -48,7 +86,7 @@ struct Gate {
 // changed nothing but Lamport times (serf/delegate.rs:495-510: status_time creeps by design); with injectors on nothing merged
 // (stale entries stay in flight forever).
 __host__ __device__ inline bool quiescent_row(const u64* row, u32 t, bool future_ops, u32 pp, bool byz_on) {
-  const u64 edges = row[1], changed = row[3], pending = row[4];
+  const u64 edges = row[ROW_EDGES], changed = row[ROW_CHANGED], pending = row[ROW_PENDING];
   const bool pp_ok = !pp || (((t + 1) % pp) == 0 && changed == 0);
   const bool byz_ok = !byz_on || changed == 0;
   return pending == 0 && edges == 0 && !future_ops && pp_ok && byz_ok;
@@ -160,10 +198,20 @@ constexpr u32 SV_OFF = 0, SV_GENERAL = 1, SV_SINGLE = 2, SV_CHECK = 3, SV_PASS =
 // at the start of the tick (its earlier pass rewrote busy bit 3 / node_due exactly), an earlier pass visited it.
 constexpr u32 CARRY_PK = 0xfu, CARRY_AWAKE = 0x10u, CARRY_TDUE = 0x20u, CARRY_SEEN = 0x40u, CARRY_TICKS = 1u << 24;
 constexpr u32 NO_DEADLINE = 0xffffffffu;
+// The set of views that can have business in `tick`, as the tick kernels publish it (W: u32 or volatile u32)
+template <class W>
+SFS_HD u32 views_of_tick(W* sched, u32 tick) { return tick >= sched[SCHED_VIEWS_FROM] ? sched[SCHED_VIEWS_NEW] : sched[SCHED_VIEWS_OLD]; }
 // A tick is skipped (grid-uniform decision of its first instruction) when the last executed tick proved that nothing can happen
 // before SCHED_IDLE_UNTIL and the host scheduled no operation for it.
 __device__ __forceinline__ bool tick_is_idle(const u32* sched, u32 tick, u32 ev_begin, u32 ev_end) {
   return sched && ev_begin == ev_end && tick < sched[SCHED_IDLE_UNTIL];
+}
+// The host operation of node v this tick (at most one; the mark kernel set its busy bit BUSY_OP), 0 if none.  P: TickParams or UeParams.
+template <class P>
+__device__ __forceinline__ u32 host_op_of(const P& p, u32 v, u32& op_slot) {
+  for (u32 e = p.ev_begin; e < p.ev_end; ++e)
+    if (p.ev_node[e] == v) { op_slot = p.ev_slot[e]; return p.ev_op[e]; }
+  return 0;
 }
 
 // Control block of a rank (one allocation, mapped into every peer): per exchange parity the entry counts and epoch flags
@@ -196,7 +244,7 @@ struct DrainParams {
   u32 byz_on, byz_delta, shard_size;
   const uint4* rec; const u64* node_state;
   u8* const* peer_anomaly;    // [world] every rank's sender-flag array
-  // user-event entries (kind 3: slot = tracked event, value = its Lamport time + 1); null / 0 when user events are off
+  // user-event entries (KIND_EXTRA: slot = tracked event, value = its Lamport time + 1); null / 0 when user events are off
   u32 ue_n;
   u32* ue_inbox_wr;
   u32* ue_ltime;
@@ -248,7 +296,7 @@ struct UeParams {
   u32* overflow;
   u32* sched;                 // scheduler words of the membership kernel (idle-tick skipping): this kernel reports its activity there
   Gate gate;                  // the user-event kernel is the first kernel of a tick when user events are on
-  // sharded runs: a target outside [first, first + n_local) gets one window entry per event (kind 3) over NVLink
+  // sharded runs: a target outside [first, first + n_local) gets one window entry per event (KIND_EXTRA) over NVLink
   u32 world, rank, shard_size, win_cap;
   u64* const* win_data;       // [world] peers' receive windows of this exchange parity
   u32* send_count;            // [world] entries written into each peer's window this tick (shared with the tick kernel)
@@ -271,7 +319,7 @@ struct ByzParams {
   u8* anomaly;                // [n_local] sender flags
   u64* totals;                // 0 injected entries, 1 injected (peer, subject) pairs
   // sharded runs: a peer in another shard gets a TRIPLE of window entries — serf entry and memberlist entry, both with
-  // BYZ_FLAG set in the destination field, then an annotation (kind 3, slot 15) carrying the sender's global id + 1 —
+  // BYZ_FLAG set in the destination field, then an annotation (KIND_EXTRA, slot 15) carrying the sender's global id + 1 —
   // and the receiving shard's drain kernel judges it against ITS record and raises the flag in the sender's shard.
   u32 n_local, world, rank, shard_size, win_cap;
   u64* const* win_data;

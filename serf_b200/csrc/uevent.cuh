@@ -152,29 +152,12 @@ __host__ __device__ inline u64 ue_hash(u64 idx, const uint4& w) {
 }
 
 
-// Gossip peers of node v at tick t — the SAME draw the membership tick kernel makes (tick_kernel.cu pick_targets:
-// one Philox4x32-10 block keyed (seed; tick, node, 0, DOMAIN_GOSSIP), rank-based sampling without replacement of
-// min(fanout, deg) neighbour slots, self slots dropped, draw order kept): user events ride in the same packets.
-__host__ __device__ inline u32 ue_draw16(const u32 (&w)[4], u32 i) { const u32 x = w[(i >> 1) & 3]; return (i & 1) ? (x >> 16) : (x & 0xffffu); }
+// Gossip peers of node v at tick t: the draw every sender makes (record.cuh peer_issue), user events ride in the same packets.
 __host__ __device__ inline u32 ue_pick_targets(u32 tick, u32 v, u32 row0, u32 deg, u32 fanout, u32 seed_lo, u32 seed_hi, const u32* col, u32 (&tg)[MAX_FANOUT]) {
-  const u32 m = fanout < deg ? fanout : deg;
-  if (!m) return 0;
-  u32 w[4];
-  philox4x32_10(tick, v, 0, DOMAIN_GOSSIP, seed_lo, seed_hi, w);
-  u32 chosen[MAX_FANOUT];                                    // ascending
-  u32 nc = 0, nt = 0;
-  for (u32 k = 0; k < m; ++k) {
-    u32 j = (ue_draw16(w, k) * (deg - k)) >> 16;
-    for (u32 i = 0; i < nc; ++i) if (j >= chosen[i]) ++j;    // rank → slot: skip the slots already taken
-    u32 pos = nc;
-    while (pos > 0 && chosen[pos - 1] > j) { chosen[pos] = chosen[pos - 1]; --pos; }
-    chosen[pos] = j; ++nc;
-    const u32 c = col[row0 + j];
-    if (c != v) tg[nt++] = c;
-  }
-  return nt;
+  u32 cand[MAX_FANOUT];
+  peer_issue<(int)MAX_FANOUT>(tick, v, fanout, seed_lo, seed_hi, row0, deg, [&](u32 e) { return col[e]; }, cand);
+  return peer_finish<(int)MAX_FANOUT>(v, cand, tg);
 }
-
 
 // Phases R and E of one node (pure): arrived events by ascending index, then the node's own injection.
 // Returns the Lamport time stamped by an injection (valid when op == OP_USER_EVENT and the node is up).

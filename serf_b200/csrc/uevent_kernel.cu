@@ -40,16 +40,13 @@ __global__ void __launch_bounds__(UE_BLOCK) uevent_kernel(const __grid_constant_
     const u32 busy = p.busy[vl];
     const uint4 w0 = p.state[vl];
     const bool queued = (w0.z | w0.w) != 0;
-    if (!TRACE && !arrived && !(busy & 2u) && !queued) continue;
+    if (!TRACE && !arrived && !(busy & BUSY_OP) && !queued) continue;
     UeRec r;
     ue_unpack(w0, r);
     const u64 ns = p.node_state[vl];
-    const bool up_r = (ns & NS_UP) != 0;
+    const bool up_r = nw_up(ns);
     u32 op = 0, op_slot = 0;
-    if (busy & 2u) {
-      for (u32 e = p.ev_begin; e < p.ev_end; ++e)
-        if (p.ev_node[e] == v) { op = p.ev_op[e]; op_slot = p.ev_slot[e]; break; }
-    }
+    if (busy & BUSY_OP) op = host_op_of(p, v, op_slot);
     bool up_s = up_r;
     if (op == OP_FAIL) up_s = false;
     if (op == OP_REJOIN) up_s = true;
@@ -71,15 +68,12 @@ __global__ void __launch_bounds__(UE_BLOCK) uevent_kernel(const __grid_constant_
         c.edges++;
         const u32 dl = tg[k] - p.first;
         if (p.world == 1 || dl < p.n_local) { atomicOr(p.inbox_wr + dl, bits[k]); continue; }
-        // another shard owns the target: one 8-byte entry per event into its window (kind 3, slot = event, value = ltime + 1)
+        // another shard owns the target: one 8-byte entry per event into its window (slot = event, value = ltime + 1)
         const u32 shard = tg[k] / p.shard_size, dloc = tg[k] - shard * p.shard_size;
         for (u32 e = 0; e < p.table.n; ++e) {
           if (!((bits[k] >> e) & 1u)) continue;
           const u32 Le = (stamped && e == op_slot) ? L : p.ltime[e];
-          const u64 entry = ((u64)(Le + 1u) << 32) | ((u64)e << 28) | (3ull << 26) | dloc;
-          const u32 g = atomicAdd(p.send_count + shard, 1u);
-          if (g < p.win_cap) p.win_data[shard][(size_t)p.rank * p.win_cap + g] = entry;
-          else *p.overflow = 2;
+          win_append<1>(p, shard, {win_entry(Le + 1u, e, KIND_EXTRA, dloc)});
           wrote_remote = true;
         }
       }
@@ -98,15 +92,15 @@ __global__ void __launch_bounds__(UE_BLOCK) uevent_kernel(const __grid_constant_
   const u64 s_hash = TRACE ? ue_warp_sum64(hash) : 0;
   if (lane == 0) {
     typedef unsigned long long ull;
-    if (s_edges) { atomicAdd((ull*)(p.row + 1), (ull)s_edges); atomicAdd((ull*)(p.totals + 1), (ull)s_edges); }
-    if (s_msgs) { atomicAdd((ull*)(p.row + 2), (ull)s_msgs); atomicAdd((ull*)(p.totals + 0), (ull)s_msgs); }
-    if (s_chg) atomicAdd((ull*)(p.row + 3), (ull)s_chg);
-    if (s_pend) atomicAdd((ull*)(p.row + 4), (ull)s_pend);
+    if (s_edges) { atomicAdd((ull*)(p.row + ROW_EDGES), (ull)s_edges); atomicAdd((ull*)(p.totals + 1), (ull)s_edges); }
+    if (s_msgs) { atomicAdd((ull*)(p.row + ROW_MESSAGES), (ull)s_msgs); atomicAdd((ull*)(p.totals + 0), (ull)s_msgs); }
+    if (s_chg) atomicAdd((ull*)(p.row + ROW_CHANGED), (ull)s_chg);
+    if (s_pend) atomicAdd((ull*)(p.row + ROW_PENDING), (ull)s_pend);
     if (s_pend | s_msgs) atomicAdd(p.sched + SCHED_UE_ACTIVITY, 1u);      // queued or sent events: the next tick cannot be skipped
     if (s_deliv) atomicAdd((ull*)(p.totals + 2), (ull)s_deliv);
     if (s_dup) atomicAdd((ull*)(p.totals + 3), (ull)s_dup);
     if (s_old) atomicAdd((ull*)(p.totals + 4), (ull)s_old);
-    if (TRACE && s_hash) atomicAdd((ull*)(p.row + 7), (ull)s_hash);
+    if (TRACE && s_hash) atomicAdd((ull*)(p.row + ROW_HASH), (ull)s_hash);
   }
 }
 

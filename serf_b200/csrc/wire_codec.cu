@@ -71,14 +71,13 @@ __device__ __forceinline__ u32 ring_len(u32 seen, const u32* lt, const u32* off)
 // lt: the tracked events' Lamport times (nullptr: no content table)
 __device__ __forceinline__ u32 pp_payload_len(const WireView& v, u32 vl, const u32* lt, NodeState* st_out, u64* sts) {
   NodeState st{};
-  st.ltime = v.node_state[vl] & 0xffffffffull;
+  st.ltime = nw_clock(v.node_state[vl]);
   st.event_ltime = v.ue_state ? v.ue_state[vl].x : 1u;
   st.seen = lt ? (v.ue_state[vl].y & ((1u << v.ue.n) - 1u)) : 0u;
   u32 len = 1 + w::varint_len(st.ltime);
   for (u32 s = 0; s < v.R; ++s) {
-    const size_t idx = (size_t)s * v.stride + vl;
     Rec r;
-    unpack(v.rec[2 * idx], v.rec[2 * idx + 1], r);
+    unpack(load_rec(v.rec, (size_t)s * v.stride + vl), r);
     if (!(r.flags & FLAG_KNOWN)) continue;
     st.known |= 1u << s;
     if (sts) sts[s] = r.st;
