@@ -37,8 +37,8 @@ extern "C" {
 #define SERFSIM_OK            0
 #define SERFSIM_E_INVAL      (-1)   /* bad argument / bad state                          */
 #define SERFSIM_E_NO_DEVICE  (-2)   /* no CUDA device / kernels not loadable             */
-#define SERFSIM_E_CUDA       (-3)   /* CUDA runtime error (text in serfsim_last_error)   */
-#define SERFSIM_E_NOMEM      (-4)
+#define SERFSIM_E_CUDA       (-3)   /* CUDA runtime error other than an allocation failure (text in serfsim_last_error) */
+#define SERFSIM_E_NOMEM      (-4)   /* a device, pinned host, stream or event allocation failed (cudaErrorMemoryAllocation) */
 #define SERFSIM_E_OVERFLOW   (-5)   /* a Lamport time / incarnation left the u32 device range */
 #define SERFSIM_E_COMM       (-6)   /* multi-GPU exchange setup failed                   */
 

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libserfsim.so")
 SOURCES = ["serfsim.cu", "tick_kernel.cu", "uevent_kernel.cu", "byz_kernel.cu", "wire_codec.cu"]
-HEADERS = ["record.cuh", "uevent.cuh", "byz.cuh", "tick_kernel.cuh", "wire.cuh", os.path.join("..", "..", "include", "serfsim.h")]
+HEADERS = ["owned.cuh", "record.cuh", "uevent.cuh", "byz.cuh", "tick_kernel.cuh", "wire.cuh", os.path.join("..", "..", "include", "serfsim.h")]
 
 
 def nvcc_path():

@@ -12,11 +12,14 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
+#include <optional>
 #include <string>
 #include <unordered_set>
 #include <vector>
 
 #include "../../include/serfsim.h"
+#include "owned.cuh"
 #include "tick_kernel.cuh"
 #include "wire.cuh"
 
@@ -34,13 +37,6 @@ namespace {
 thread_local std::string g_err;
 
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
-
-#define CU(call)                                                                              \
-  do {                                                                                        \
-    cudaError_t e_ = (call);                                                                  \
-    if (e_ != cudaSuccess)                                                                    \
-      return fail(SERFSIM_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_));        \
-  } while (0)
 
 struct HostOp { u32 tick, op, node, slot; u64 seq; };
 
@@ -167,58 +163,57 @@ struct serfsim {
   u32 N = 0, R = 0, first = 0, count = 0, shard_size = 0;
   u32 stride = 0;                  // count rounded up to a whole 256-node tile: stride of every per-slot plane
   Rules rules{};
+  Stream stream;                   // declared before every buffer: destroyed after them
+  Event ev0, ev1;
   // device state
-  uint4* d_rec = nullptr;          // [R][stride] × 32 B (transmit-budget bytes zero)
-  u32* d_qword = nullptr;          // [R][stride] queue words (transmit budgets)
-  u32* d_inbox[2] = {nullptr, nullptr};   // [3][R][count]
-  u64* d_node = nullptr;           // [count]
-  u8* d_busy = nullptr;            // [stride] per-node busy byte
-  u16* d_watch = nullptr;          // [stride] per-node watcher mask (subjects among the node's neighbours)
+  DevArray<uint4> d_rec;           // [R][stride] × 32 B (transmit-budget bytes zero)
+  DevArray<u32> d_qword;           // [R][stride] queue words (transmit budgets)
+  DevArray<u32> d_inbox[2];        // [3][R][stride]
+  DevArray<u64> d_node;            // [stride]
+  DevArray<u8> d_busy;             // [stride] per-node busy byte
+  DevArray<u16> d_watch;           // [stride] per-node watcher mask (subjects among the node's neighbours)
   bool watch_dirty = true;
-  uint4* d_snap_rec = nullptr;     // push-pull rounds: end-of-tick snapshot of the records …
-  u64* d_snap_node = nullptr;      // … and of the node words
-  const uint4** d_peer_snap_rec = nullptr;   // sharded push-pull: device arrays of every rank's snapshot pointers
-  const u64** d_peer_snap_node = nullptr;
-  u8* d_hot[2] = {nullptr, nullptr};      // [n_tiles] per tick parity
-  u8* d_hot_static = nullptr;             // [n_tiles] tiles that hold a watcher (never consumed)
-  u32* d_node_due = nullptr;              // [stride] per-node earliest suspicion deadline (tick_kernel.cuh)
-  u32* d_carry = nullptr;                 // [stride] per-view passes: carry words (tick_kernel.cuh: CARRY_*); unsharded multi-slot runs only
-  u32* d_tile_due = nullptr;              // [n_tiles] earliest suspicion deadline of a tile's nodes (the timer wheel)
-  u32* d_sched = nullptr;                 // scheduler words (tick_kernel.cuh: SCHED_*)
+  DevArray<uint4> d_snap_rec;      // push-pull rounds (allocated by serfsim_create): end-of-tick snapshot of the records …
+  DevArray<u64> d_snap_node;       // … and of the node words
+  DevArray<const uint4*> d_peer_snap_rec;   // sharded push-pull: device arrays of every rank's snapshot pointers
+  DevArray<const u64*> d_peer_snap_node;
+  DevArray<u8> d_hot[2];                  // [n_tiles] per tick parity
+  DevArray<u8> d_hot_static;              // [n_tiles] tiles that hold a watcher (never consumed)
+  DevArray<u32> d_node_due;               // [stride] per-node earliest suspicion deadline (tick_kernel.cuh)
+  DevArray<u32> d_carry;                  // [stride] per-view passes: carry words (tick_kernel.cuh: CARRY_*); unsharded multi-slot runs only
+  DevArray<u32> d_tile_due;               // [n_tiles] earliest suspicion deadline of a tile's nodes (the timer wheel)
+  DevArray<u32> d_sched;                  // scheduler words (tick_kernel.cuh: SCHED_*)
   u32 n_tiles = 0;
-  u32* d_rowptr = nullptr;         // [count+1]
-  u32* d_col = nullptr;
-  u32 *d_ev_node = nullptr, *d_ev_op = nullptr, *d_ev_slot = nullptr;
+  DevArray<u32> d_rowptr;          // [stride+8]
+  DevArray<u32> d_col;
+  DevArray<u32> d_ev_node, d_ev_op, d_ev_slot;
   size_t ev_cap = 0;
-  u64* d_trace = nullptr;          // [trace_cap][8]
-  u32* d_kinds = nullptr;          // [trace_cap+1][4]; row t+1 = messages by kind sent in tick t
-  u32* d_view_kinds = nullptr;     // [trace_cap+1][R][4]; row t+1 = messages by view and kind sent in tick t by per-view passes (zero otherwise)
+  DevArray<u64> d_trace;           // [trace_cap][8]
+  DevArray<u32> d_kinds;           // [trace_cap+1][4]; row t+1 = messages by kind sent in tick t
+  DevArray<u32> d_view_kinds;      // [trace_cap+1][R][4]; row t+1 = messages by view and kind sent in tick t by per-view passes (zero otherwise)
   u32 trace_cap = 0;
-  u32* d_overflow = nullptr;       // device address of pin_overflow (mapped pinned host memory: written by kernels on the rare error paths, read by the host without a copy)
-  u32* pin_overflow = nullptr;
-  u32* d_subj = nullptr;
-  u64* d_scratch = nullptr;        // summary / hash output
-  void* d_stage = nullptr;         // getter staging, count × 8 B
-  // user events (SURVEY §8f row 3): allocated by serfsim_set_user_events
+  MappedWords pin_overflow;        // written by kernels on the rare error paths, read by the host without a copy
+  u32* d_overflow = nullptr;       // its device address
+  DevArray<u32> d_subj;
+  DevArray<u64> d_scratch;         // summary / hash output
+  DevArray<u64> d_stage;           // getter staging, count × 8 B
+  // user events (SURVEY §8f row 3), allocated together by serfsim_set_user_events: [stride] 16-byte event records and arrived-event
+  // masks per tick parity, [MAX_UEVENTS] Lamport times, [8] totals; push-pull rounds: the record snapshot partners read, and every rank's
+  struct UserEvents { DevArray<uint4> state, snap; DevArray<u32> inbox[2], ltime; DevArray<u64> totals; DevArray<const uint4*> peer_snap; };
+  std::optional<UserEvents> ue;
   UeTable ue_table{};              // n = 0: user events off
-  uint4* d_ue_state = nullptr;     // [stride] 16-byte event records
-  u32* d_ue_inbox[2] = {nullptr, nullptr};   // [stride] arrived-event masks per tick parity
-  u32* d_ue_ltime = nullptr;       // [MAX_UEVENTS]
   wire::UeWire ue_wire{};          // wire form of the tracked events (serfsim_set_user_event_content); n = 0: none
-  u8* d_ue_entries = nullptr;      // its UserEvents.events entries on the device
-  u64* d_ue_totals = nullptr;      // [8]
+  DevArray<u8> d_ue_entries;       // its UserEvents.events entries on the device
   u32 ue_injected = 0;             // tracked events already scheduled (each may be injected once)
-  uint4* d_ue_snap = nullptr;      // push-pull rounds: snapshot of the event records (partners read it)
-  const uint4** d_peer_ue_snap = nullptr;
   u32 ue_origin[MAX_UEVENTS] = {0};
   u32 ue_fire_tick[MAX_UEVENTS] = {0};  // origin node of each scheduled event (its shard is the one that stamps the Lamport time)
-  // byzantine injectors (BASELINE configs[4]): allocated by serfsim_set_byzantine
+  // byzantine injectors (BASELINE configs[4]): allocated by serfsim_set_byzantine (sharded runs: by serfsim_create, peers raise the
+  // flags): [stride] sender flags, [4] totals, [byz_n] ascending ids
   u32 byz_n = 0, byz_delta = 2;    // byz_n: injectors of THIS shard
   bool byz_on = false;             // any injector anywhere (all ranks agree): changes the convergence rule and the drain kernel
-  u8** d_peer_anomaly = nullptr;   // sharded runs: device array of every rank's flag array
-  u32* d_byz_ids = nullptr;        // [byz_n] ascending
-  u8* d_anomaly = nullptr;         // [stride] sender flags
-  u64* d_byz_totals = nullptr;     // [4]
+  struct Injectors { DevArray<u8> anomaly; DevArray<u64> totals; DevArray<u32> ids; };
+  std::optional<Injectors> byz;
+  DevArray<u8*> d_peer_anomaly;    // sharded runs: device array of every rank's flag array
   // host state
   std::vector<HostOp> ops;         // sorted by (tick, seq)
   std::unordered_set<u64> op_keys; // (tick << 32 | node): at most one operation per node per tick
@@ -235,16 +230,14 @@ struct serfsim {
   u32 udeg = 0;                    // uniform out-degree of the shard's rows (0: degrees differ)
   std::vector<serfsim_tick_row_t> rows;   // rows pulled from the device so far (global sums when sharded)
   // device-side convergence gate (tick_kernel.cuh: Gate)
-  u32* d_runctl = nullptr;         // [0] done flag, [1] first quiescent tick
-  u32* pin_ctl = nullptr;          // the verdict in mapped pinned host memory (written by the gate's leader thread), read once per chunk
+  DevArray<u32> d_runctl;          // [0] done flag, [1] first quiescent tick
+  MappedWords pin_ctl;             // [4] the verdict, written by the gate's leader thread and read once per chunk
   u32* d_pin_ctl = nullptr;        // its device address
-  u64* d_grow = nullptr;           // sharded runs: [trace_cap][8] global trace rows, summed on the device by the drain kernel
+  DevArray<u64> d_grow;            // sharded runs: [trace_cap][8] global trace rows, summed on the device by the drain kernel
   bool gate_on = false;
   u32 gate_first = 0;              // first tick of the current run_until_converged call (it always runs)
   std::vector<u32> launch_log;     // kernels launched per tick since the timing window opened (ticks past the quiescent one do not count)
   u32 launch_log_first = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   bool timing_open = false;
   double last_ms = 0.0;
   u64 last_launches = 0, launches = 0;
@@ -256,29 +249,27 @@ struct serfsim {
   int sms = 132;                   // the device's SM count
   Switches sw;                     // run-time switches, read at serfsim_create
   // multi-GPU
-  u64* d_win_data[2] = {nullptr, nullptr};     // my receive windows [parity][world][win_cap]  (IPC-exported)
-  u32* d_ctrl = nullptr;                       // my control block [parity][counts[8] | flags[8]] (IPC-exported)
-  u32* d_send_count = nullptr;                 // [world] entries written into each peer's window this tick
-  u64** d_peer_data[2] = {nullptr, nullptr};   // device arrays of peer window pointers, per parity
-  u32** d_peer_ctrl = nullptr;                 // device array of peer control-block pointers
+  DevArray<u64> d_win_data[2];                 // my receive windows [parity][world][win_cap]  (IPC-exported)
+  DevArray<u32> d_ctrl;                        // my control block [parity][counts[8] | flags[8]] (IPC-exported)
+  DevArray<u32> d_send_count;                  // [world] entries written into each peer's window this tick
+  DevArray<u64*> d_peer_data[2];               // device arrays of peer window pointers, per parity
+  DevArray<u32*> d_peer_ctrl;                  // device array of peer control-block pointers
   u32 xepoch = 0;                              // executed-tick counter of the exchange (never rewinds): stamps and parity
   u32 win_cap = 0;
   u32 win_cap_base = 0;                        // capacity sized for the membership entries alone (serfsim_create)
   bool connected = false;
   bool loopback = false;                       // serfsim_comm_loopback: profiling aid, the handle exchanges with itself
   serfsim_barrier_fn barrier = nullptr; serfsim_allreduce_u64_fn allreduce = nullptr; void* comm_user = nullptr;
-  std::vector<void*> ipc_opened;
+  std::vector<IpcMapping> ipc_opened;
   bool tick_timing = false;
   size_t l2_persist_max = 0, l2_window_max = 0;
   // asynchronous result read-back (serfsim_results_async): extraction into a ring of staging buffers on the launch stream,
   // device→host copies on a second stream so that they overlap the ticks of the caller's next step
-  struct ResBuf { unsigned char* d = nullptr; cudaEvent_t copied = nullptr; bool used = false; };
-  ResBuf res[4];
-  u32 res_next = 0;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_extracted = nullptr;
-  std::vector<cudaEvent_t> tick_ev;      // 2 per tick when tick_timing
-  std::vector<cudaEvent_t> mid_ev;       // after the tick kernel (multi-GPU breakdown, SERFSIM_XTIMING=1)
+  struct ResBuf { DevArray<unsigned char> d; Event copied; bool used = false; };
+  struct ReadBack { Stream copy_stream; Event extracted; ResBuf res[4]; u32 next = 0; };
+  std::optional<ReadBack> rb;      // allocated together by the first serfsim_results_async
+  std::vector<Event> tick_ev;      // 2 per tick when tick_timing
+  std::vector<Event> mid_ev;       // after the tick kernel (multi-GPU breakdown, SERFSIM_XTIMING=1)
 };
 
 namespace {
@@ -292,24 +283,11 @@ int ensure_trace(serfsim* h, u32 need) {
   if (need <= h->trace_cap) return 0;
   u32 cap = std::max<u32>(1024, h->trace_cap);
   while (cap < need) cap *= 2;
-  u64* nt = nullptr; u32* nk = nullptr; u32* nv = nullptr; u64* ng = nullptr;
-  const bool sharded = h->cfg.world_size > 1;
-  CU(cudaMalloc(&nt, (size_t)cap * sizeof(serfsim_tick_row_t)));
-  CU(cudaMalloc(&nk, ((size_t)cap + 1) * 4 * sizeof(u32)));
-  CU(cudaMalloc(&nv, ((size_t)cap + 1) * h->R * 4 * sizeof(u32)));
-  CU(cudaMemsetAsync(nt, 0, (size_t)cap * sizeof(serfsim_tick_row_t), h->stream));
-  CU(cudaMemsetAsync(nk, 0, ((size_t)cap + 1) * 4 * sizeof(u32), h->stream));
-  CU(cudaMemsetAsync(nv, 0, ((size_t)cap + 1) * h->R * 4 * sizeof(u32), h->stream));
-  if (sharded) { CU(cudaMalloc(&ng, (size_t)cap * sizeof(serfsim_tick_row_t))); CU(cudaMemsetAsync(ng, 0, (size_t)cap * sizeof(serfsim_tick_row_t), h->stream)); }
-  if (h->d_trace) {
-    CU(cudaMemcpyAsync(nt, h->d_trace, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToDevice, h->stream));
-    CU(cudaMemcpyAsync(nk, h->d_kinds, ((size_t)h->trace_cap + 1) * 4 * sizeof(u32), cudaMemcpyDeviceToDevice, h->stream));
-    CU(cudaMemcpyAsync(nv, h->d_view_kinds, ((size_t)h->trace_cap + 1) * h->R * 4 * sizeof(u32), cudaMemcpyDeviceToDevice, h->stream));
-    if (sharded) CU(cudaMemcpyAsync(ng, h->d_grow, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToDevice, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds); cudaFree(h->d_grow);
-  }
-  h->d_trace = nt; h->d_kinds = nk; h->d_view_kinds = nv; h->d_grow = ng; h->trace_cap = cap;
+  CU(h->d_trace.grow((size_t)cap * ROW_FIELDS, h->stream));
+  CU(h->d_kinds.grow(((size_t)cap + 1) * 4, h->stream));
+  CU(h->d_view_kinds.grow(((size_t)cap + 1) * h->R * 4, h->stream));
+  if (h->cfg.world_size > 1) CU(h->d_grow.grow((size_t)cap * ROW_FIELDS, h->stream));
+  h->trace_cap = cap;
   return 0;
 }
 
@@ -320,8 +298,7 @@ int upload_ops(serfsim* h) {
   if (n > h->ev_cap) {
     size_t cap = std::max<size_t>(1024, h->ev_cap);
     while (cap < n) cap *= 2;
-    if (h->d_ev_node) { cudaFree(h->d_ev_node); cudaFree(h->d_ev_op); cudaFree(h->d_ev_slot); }
-    CU(cudaMalloc(&h->d_ev_node, cap * 4)); CU(cudaMalloc(&h->d_ev_op, cap * 4)); CU(cudaMalloc(&h->d_ev_slot, cap * 4));
+    CU(h->d_ev_node.alloc(cap)); CU(h->d_ev_op.alloc(cap)); CU(h->d_ev_slot.alloc(cap));
     h->ev_cap = cap;
   }
   if (n) {
@@ -389,15 +366,15 @@ TickParams at_view(const serfsim* h, const TickParams& p, u32 s) {
 }
 
 // Timing events, created on first use: ev holds at least n.
-int grow_events(std::vector<cudaEvent_t>& ev, size_t n) {
-  while (ev.size() < n) { cudaEvent_t e; CU(cudaEventCreate(&e)); ev.push_back(e); }
+int grow_events(std::vector<Event>& ev, size_t n) {
+  while (ev.size() < n) { Event e; CU(e.create()); ev.push_back(std::move(e)); }
   return 0;
 }
 
 // The tracked user events' Lamport times as the cluster knows them: the origin's shard stamps an event, the other shards may not have it
 // yet, so each contributes the stamps of its own nodes' events and every rank gets the sum (a collective when sharded).  Stream idle.
 int ue_cluster_ltimes(serfsim* h, u32 lt[MAX_UEVENTS]) {
-  CU(cudaMemcpy(lt, h->d_ue_ltime, MAX_UEVENTS * sizeof(u32), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(lt, h->ue->ltime, h->ue->ltime.bytes(), cudaMemcpyDeviceToHost));
   if (h->cfg.world_size > 1 && h->allreduce) {
     u64 v[MAX_UEVENTS];
     for (u32 e = 0; e < MAX_UEVENTS; ++e) v[e] = (((h->ue_injected >> e) & 1u) && h->ue_origin[e] - h->first < h->count) ? lt[e] : 0;
@@ -473,10 +450,10 @@ void launch_user_events(serfsim* h, const TickParams& p) {
   UeParams u{};
   u.n_local = h->count; u.first = h->first; u.n_global = h->N; u.R = h->R; u.fanout = h->cfg.fanout; u.tick = t;
   u.seed_lo = p.seed_lo; u.seed_hi = p.seed_hi; u.limit = h->rules.limit; u.ev_begin = p.ev_begin; u.ev_end = p.ev_end;
-  u.table = h->ue_table; u.state = h->d_ue_state; u.inbox_rd = h->d_ue_inbox[(t & 1) ^ 1]; u.inbox_wr = h->d_ue_inbox[t & 1];
-  u.ltime = h->d_ue_ltime; u.node_state = h->d_node; u.busy = h->d_busy; u.row_ptr = h->d_rowptr; u.col = h->d_col;
+  u.table = h->ue_table; u.state = h->ue->state; u.inbox_rd = h->ue->inbox[(t & 1) ^ 1]; u.inbox_wr = h->ue->inbox[t & 1];
+  u.ltime = h->ue->ltime; u.node_state = h->d_node; u.busy = h->d_busy; u.row_ptr = h->d_rowptr; u.col = h->d_col;
   u.ev_node = h->d_ev_node; u.ev_op = h->d_ev_op; u.ev_slot = h->d_ev_slot;
-  u.row = p.row; u.totals = h->d_ue_totals; u.overflow = h->d_overflow; u.sched = h->d_sched;
+  u.row = p.row; u.totals = h->ue->totals; u.overflow = h->d_overflow; u.sched = h->d_sched;
   u.world = p.world; u.rank = p.rank; u.shard_size = h->shard_size; u.win_cap = h->win_cap;
   u.win_data = p.win_data; u.send_count = h->d_send_count;
   u.gate = p.gate; u.gate.evaluate = 1u;
@@ -523,9 +500,9 @@ void launch_injectors(serfsim* h, const TickParams& p) {
   const u32 t = p.tick;
   ByzParams b{};
   b.n_byz = h->byz_n; b.first = h->first; b.R = h->R; b.stride = h->stride; b.fanout = h->cfg.fanout; b.tick = t;
-  b.seed_lo = p.seed_lo; b.seed_hi = p.seed_hi; b.delta = h->byz_delta; b.ids = h->d_byz_ids; b.rec = h->d_rec; b.node_state = h->d_node;
+  b.seed_lo = p.seed_lo; b.seed_hi = p.seed_hi; b.delta = h->byz_delta; b.ids = h->byz->ids; b.rec = h->d_rec; b.node_state = h->d_node;
   b.row_ptr = h->d_rowptr; b.col = h->d_col; b.inbox_wr = h->d_inbox[t & 1]; b.hot_wr = h->d_hot[t & 1]; b.kinds_cur = p.kinds_cur;
-  b.anomaly = h->d_anomaly; b.totals = h->d_byz_totals;
+  b.anomaly = h->byz->anomaly; b.totals = h->byz->totals;
   b.n_local = h->count; b.world = p.world; b.rank = p.rank; b.shard_size = h->shard_size; b.win_cap = h->win_cap;
   b.win_data = p.win_data; b.send_count = h->d_send_count; b.overflow = h->d_overflow; b.gate = p.gate.ctl;
   launch_byz(b, h->stream);
@@ -544,9 +521,9 @@ void launch_exchange(serfsim* h, const TickParams& p) {
   d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.world; d.rank = p.rank; d.win_cap = h->win_cap; d.stamp = p.stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
   d.win_data = h->d_win_data[xpar]; d.ctrl = h->d_ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
   d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = h->d_peer_anomaly;
-  d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->d_ue_inbox[t & 1] : nullptr; d.ue_ltime = h->d_ue_ltime;
+  d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->ue->inbox[t & 1].get() : nullptr; d.ue_ltime = h->ue ? h->ue->ltime.get() : nullptr;
   d.my_row = p.row; d.grow = h->d_grow + (size_t)t * ROW_FIELDS; d.gate = p.gate.ctl;
-  d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(h->d_ctrl) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
+  d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(h->d_ctrl.get()) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
   d.sched = h->d_sched; d.sched_rw = h->d_sched; d.host_idle_until = h->d_pin_ctl + 2; d.tick = t; d.sleep_on = p.sleep_on;
   launch_drain(d, h->stream);
   h->last_launches += 1;
@@ -556,14 +533,12 @@ void launch_exchange(serfsim* h, const TickParams& p) {
 // Anti-entropy round on a snapshot of the end-of-tick state (only this node's own records are written); p: as the membership tick left it.
 int anti_entropy_round(serfsim* h, TickParams p) {
   const u32 t = p.tick;
-  const size_t rb = (size_t)h->R * h->stride * 32, nb = (size_t)h->stride * 8;
-  if (!h->d_snap_rec) { CU(cudaMalloc(&h->d_snap_rec, rb)); CU(cudaMalloc(&h->d_snap_node, nb)); }
-  CU(cudaMemcpyAsync(h->d_snap_rec, h->d_rec, rb, cudaMemcpyDeviceToDevice, h->stream));
-  CU(cudaMemcpyAsync(h->d_snap_node, h->d_node, nb, cudaMemcpyDeviceToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_snap_rec, h->d_rec, h->d_rec.bytes(), cudaMemcpyDeviceToDevice, h->stream));
+  CU(cudaMemcpyAsync(h->d_snap_node, h->d_node, h->d_node.bytes(), cudaMemcpyDeviceToDevice, h->stream));
   if (h->ue_table.n) {
-    CU(cudaMemcpyAsync(h->d_ue_snap, h->d_ue_state, (size_t)h->stride * 16, cudaMemcpyDeviceToDevice, h->stream));
-    p.ue_table = h->ue_table; p.ue_state = h->d_ue_state; p.ue_snap = h->d_ue_snap; p.ue_snap_peer = h->d_peer_ue_snap;
-    p.ue_ltime = h->d_ue_ltime; p.ue_totals = h->d_ue_totals;
+    CU(cudaMemcpyAsync(h->ue->snap, h->ue->state, h->ue->state.bytes(), cudaMemcpyDeviceToDevice, h->stream));
+    p.ue_table = h->ue_table; p.ue_state = h->ue->state; p.ue_snap = h->ue->snap; p.ue_snap_peer = h->ue->peer_snap;
+    p.ue_ltime = h->ue->ltime; p.ue_totals = h->ue->totals;
   }
   if (h->cfg.world_size > 1) {
     // partners may live on other GPUs: their snapshots are read through the peer mappings.  Rounds are rare (every
@@ -578,7 +553,7 @@ int anti_entropy_round(serfsim* h, TickParams p) {
       // installs the cluster's times before the round.
       u32 lt[MAX_UEVENTS];
       if (int rc = ue_cluster_ltimes(h, lt)) return rc;
-      CU(cudaMemcpy(h->d_ue_ltime, lt, sizeof(lt), cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(h->ue->ltime, lt, h->ue->ltime.bytes(), cudaMemcpyHostToDevice));
     }
     launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
     CU(cudaStreamSynchronize(h->stream));
@@ -623,9 +598,8 @@ int launch_ticks(serfsim* h, u32 n) {
     }
     if (h->sw.l2_window && h->l2_window_max) {
       cudaStreamAttrValue av{};
-      const size_t bytes = (size_t)3 * h->R * h->stride * sizeof(u32);
       av.accessPolicyWindow.base_ptr = h->d_inbox[t & 1];
-      av.accessPolicyWindow.num_bytes = std::min(bytes, h->l2_window_max);
+      av.accessPolicyWindow.num_bytes = std::min(h->d_inbox[t & 1].bytes(), h->l2_window_max);
       av.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)h->l2_persist_max / (double)std::max<size_t>(1, av.accessPolicyWindow.num_bytes));
       av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
       av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
@@ -718,7 +692,7 @@ int refresh_watchers(serfsim* h) {
     launch_compute_watch(h->d_rowptr, h->d_col, h->d_subj, h->R, h->first, h->count, h->d_watch, h->stream);
     h->watch_dirty = false;
   }
-  CU(cudaMemsetAsync(h->d_hot_static, 0, h->n_tiles, h->stream));
+  CU(h->d_hot_static.fill(0, h->stream));
   launch_apply_watch(h->d_watch, h->count, h->d_busy, h->d_hot_static, h->stream);
   CU(cudaGetLastError());
   return 0;
@@ -727,11 +701,9 @@ int refresh_watchers(serfsim* h) {
 int ue_reset(serfsim* h) {                      // bootstrap event state: clock 1, nothing seen, nothing queued
   h->ue_injected = 0;
   if (!h->ue_table.n) return 0;
-  launch_ue_init(h->d_ue_state, h->count, h->stream);
-  CU(cudaMemsetAsync(h->d_ue_inbox[0], 0, (size_t)h->stride * 4, h->stream));
-  CU(cudaMemsetAsync(h->d_ue_inbox[1], 0, (size_t)h->stride * 4, h->stream));
-  CU(cudaMemsetAsync(h->d_ue_ltime, 0, MAX_UEVENTS * 4, h->stream));
-  CU(cudaMemsetAsync(h->d_ue_totals, 0, 8 * 8, h->stream));
+  launch_ue_init(h->ue->state, h->count, h->stream);
+  CU(h->ue->inbox[0].fill(0, h->stream)); CU(h->ue->inbox[1].fill(0, h->stream));
+  CU(h->ue->ltime.fill(0, h->stream)); CU(h->ue->totals.fill(0, h->stream));
   CU(cudaGetLastError());
   return 0;
 }
@@ -741,70 +713,33 @@ int do_reset(serfsim* h, u64 seed) {
   h->up_mask = (h->R >= 32) ? 0xffffffffu : ((1u << h->R) - 1);
   h->ever_down = 0;
   h->reported.assign(h->R, (u8)ST_ALIVE);
-  const size_t inbox_bytes = (size_t)3 * h->R * h->stride * sizeof(u32);
   launch_init_state(h->d_rec, h->d_node, h->count, h->stride, h->R, h->cfg.init_status_ltime, h->cfg.init_clock, h->stream);
-  CU(cudaMemsetAsync(h->d_inbox[0], 0, inbox_bytes, h->stream));
-  CU(cudaMemsetAsync(h->d_inbox[1], 0, inbox_bytes, h->stream));
+  CU(h->d_inbox[0].fill(0, h->stream)); CU(h->d_inbox[1].fill(0, h->stream));
   CU(cudaStreamSynchronize(h->stream));                   // no kernel of an earlier run is still writing the error word
   *(volatile u32*)h->pin_overflow = 0;
   ((volatile u32*)h->pin_ctl)[2] = 0;                     // the scheduler's "sleep until" word (mirrors d_sched, cleared below)
-  CU(cudaMemsetAsync(h->d_busy, 0, h->stride, h->stream));
-  CU(cudaMemsetAsync(h->d_qword, 0, (size_t)h->R * h->stride * 4, h->stream));
-  CU(cudaMemsetAsync(h->d_hot[0], 0, h->n_tiles, h->stream));
-  CU(cudaMemsetAsync(h->d_hot[1], 0, h->n_tiles, h->stream));
-  CU(cudaMemsetAsync(h->d_tile_due, 0xff, (size_t)h->n_tiles * sizeof(u32), h->stream));      // no timer runs
-  CU(cudaMemsetAsync(h->d_node_due, 0xff, (size_t)h->stride * sizeof(u32), h->stream));
-  if (h->d_carry) CU(cudaMemsetAsync(h->d_carry, 0, (size_t)h->stride * sizeof(u32), h->stream));   // tags restart with the ticks
-  CU(cudaMemsetAsync(h->d_sched, 0, SCHED_WORDS * sizeof(u32), h->stream));
-  if (h->d_trace) {
-    CU(cudaMemsetAsync(h->d_trace, 0, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), h->stream));
-    CU(cudaMemsetAsync(h->d_kinds, 0, ((size_t)h->trace_cap + 1) * 4 * sizeof(u32), h->stream));
-    CU(cudaMemsetAsync(h->d_view_kinds, 0, ((size_t)h->trace_cap + 1) * h->R * 4 * sizeof(u32), h->stream));
-  }
-  if (h->d_grow) CU(cudaMemsetAsync(h->d_grow, 0, (size_t)h->trace_cap * sizeof(serfsim_tick_row_t), h->stream));
-  CU(cudaMemsetAsync(h->d_runctl, 0, 2 * sizeof(u32), h->stream));
-  if (h->d_send_count) CU(cudaMemsetAsync(h->d_send_count, 0, sizeof(u32) * 8, h->stream));
+  CU(h->d_busy.fill(0, h->stream)); CU(h->d_qword.fill(0, h->stream));
+  CU(h->d_hot[0].fill(0, h->stream)); CU(h->d_hot[1].fill(0, h->stream));
+  CU(h->d_tile_due.fill(0xff, h->stream)); CU(h->d_node_due.fill(0xff, h->stream));      // no timer runs
+  CU(h->d_carry.fill(0, h->stream));                     // tags restart with the ticks
+  CU(h->d_sched.fill(0, h->stream));
+  CU(h->d_trace.fill(0, h->stream)); CU(h->d_kinds.fill(0, h->stream)); CU(h->d_view_kinds.fill(0, h->stream)); CU(h->d_grow.fill(0, h->stream));
+  CU(h->d_runctl.fill(0, h->stream)); CU(h->d_send_count.fill(0, h->stream));
   { int rc = ue_reset(h); if (rc) return rc; }
-  if (h->d_anomaly) { CU(cudaMemsetAsync(h->d_anomaly, 0, h->stride, h->stream)); CU(cudaMemsetAsync(h->d_byz_totals, 0, 4 * 8, h->stream)); }
+  if (h->byz) { CU(h->byz->anomaly.fill(0, h->stream)); CU(h->byz->totals.fill(0, h->stream)); }
   { int rc = refresh_watchers(h); if (rc) return rc; }
   CU(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
-void free_all(serfsim* h) {
-  for (void* p : h->ipc_opened) cudaIpcCloseMemHandle(p);
-  for (cudaEvent_t e : h->tick_ev) cudaEventDestroy(e);
-  cudaFree(h->d_hot_static); cudaFree(h->d_tile_due); cudaFree(h->d_node_due); cudaFree(h->d_carry); cudaFree(h->d_sched);
-  cudaFree(h->d_hot[0]); cudaFree(h->d_hot[1]); cudaFree(h->d_busy); cudaFree(h->d_watch); cudaFree(h->d_snap_rec); cudaFree(h->d_snap_node); cudaFree(h->d_peer_snap_rec); cudaFree(h->d_peer_snap_node);
-  cudaFree(h->d_qword);
-  cudaFree(h->d_rec); cudaFree(h->d_inbox[0]); cudaFree(h->d_inbox[1]); cudaFree(h->d_node); cudaFree(h->d_rowptr); cudaFree(h->d_col);
-  cudaFree(h->d_ev_node); cudaFree(h->d_ev_op); cudaFree(h->d_ev_slot); cudaFree(h->d_trace); cudaFree(h->d_kinds); cudaFree(h->d_view_kinds);
-  if (h->pin_overflow) cudaFreeHost(h->pin_overflow);
-  cudaFree(h->d_subj); cudaFree(h->d_scratch); cudaFree(h->d_stage);
-  cudaFree(h->d_byz_ids); cudaFree(h->d_anomaly); cudaFree(h->d_byz_totals); cudaFree(h->d_peer_anomaly);
-  cudaFree(h->d_ue_snap); cudaFree(h->d_peer_ue_snap);
-  cudaFree(h->d_ue_entries);
-  cudaFree(h->d_ue_state); cudaFree(h->d_ue_inbox[0]); cudaFree(h->d_ue_inbox[1]); cudaFree(h->d_ue_ltime); cudaFree(h->d_ue_totals);
-  for (int par = 0; par < 2; ++par) { cudaFree(h->d_win_data[par]); cudaFree(h->d_peer_data[par]); }
-  cudaFree(h->d_ctrl); cudaFree(h->d_send_count); cudaFree(h->d_peer_ctrl);
-  for (auto& b : h->res) { cudaFree(b.d); if (b.copied) cudaEventDestroy(b.copied); }
-  if (h->ev_extracted) cudaEventDestroy(h->ev_extracted);
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  if (h->pin_ctl) cudaFreeHost(h->pin_ctl);
-  cudaFree(h->d_runctl); cudaFree(h->d_grow);
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
-  if (h->stream) cudaStreamDestroy(h->stream);
-}
-
-// A peer's exported buffer mapped into this process (unmapped by free_all).
+// A peer's exported buffer mapped into this process (unmapped when the handle is destroyed).
 template <class T>
 int ipc_open(serfsim* h, const cudaIpcMemHandle_t& handle, const char* what, T** out) {
-  void* ptr = nullptr;
-  const cudaError_t e = cudaIpcOpenMemHandle(&ptr, handle, cudaIpcMemLazyEnablePeerAccess);
+  IpcMapping m;
+  const cudaError_t e = m.create(handle);
   if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(") + what + "): " + cudaGetErrorString(e));
-  h->ipc_opened.push_back(ptr);
-  *out = (T*)ptr;
+  *out = (T*)(void*)m;
+  h->ipc_opened.push_back(std::move(m));
   return 0;
 }
 
@@ -825,8 +760,8 @@ struct WireView { const uint4* rec; const u32* qword; const u64* node_state; con
 int serfsim_fail(int code, const char* msg) { return fail(code, msg); }
 int serfsim_wire_view(const serfsim* h, WireView* out) {
   if (!h) return fail(SERFSIM_E_INVAL, "null handle");
-  *out = WireView{h->d_rec, h->d_qword, h->d_node, h->ue_table.n ? h->d_ue_state : nullptr, h->d_subj, h->count, h->stride, h->R, h->stream, h->ue_wire};
-  out->ue.ltime = h->d_ue_ltime;
+  *out = WireView{h->d_rec, h->d_qword, h->d_node, h->ue_table.n ? h->ue->state.get() : nullptr, h->d_subj, h->count, h->stride, h->R, h->stream, h->ue_wire};
+  out->ue.ltime = h->ue ? h->ue->ltime.get() : nullptr;
   return 0;
 }
 }  // namespace sfs
@@ -888,13 +823,13 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   CU(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
   if (major != 9 || minor != 0) return fail(SERFSIM_E_NO_DEVICE, "kernels are built for sm_90a only (H100)");
 
-  serfsim* h = new serfsim();
+  std::unique_ptr<serfsim> h(new serfsim());
   h->cfg = *cfg; h->N = cfg->n_nodes; h->R = cfg->slots;
   h->shard_size = (h->N + cfg->world_size - 1) / cfg->world_size;
   h->first = std::min<u64>((u64)h->shard_size * cfg->rank, h->N);
   h->count = (u32)std::min<u64>(h->shard_size, (u64)h->N - h->first);
-  if (h->count == 0) { delete h; return fail(SERFSIM_E_INVAL, "empty shard"); }
-  if (h->shard_size >= (1u << 26)) { delete h; return fail(SERFSIM_E_INVAL, "shard larger than 2^26 nodes"); }
+  if (h->count == 0) return fail(SERFSIM_E_INVAL, "empty shard");
+  if (h->shard_size >= (1u << 26)) return fail(SERFSIM_E_INVAL, "shard larger than 2^26 nodes");
   h->rules.limit = (u32)retransmit_limit(cfg->retransmit_mult, h->N);      // 1..255: checked above
   auto tab = suspicion_table(cfg->suspicion_mult, cfg->suspicion_max_timeout_mult, cfg->probe_interval_ticks ? cfg->probe_interval_ticks : 1, cfg->gossip_interval_ms, h->N);
   h->rules.k = (u32)tab.size() - 1;
@@ -902,38 +837,27 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   h->subj.resize(h->R);
   for (u32 s = 0; s < h->R; ++s) h->subj[s] = s;
 
-  auto bail = [&](int rc) { free_all(h); delete h; return rc; };
-#define CUB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return bail(fail(e_ == cudaErrorMemoryAllocation ? SERFSIM_E_NOMEM : SERFSIM_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_))); } while (0)
-  CUB(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  CUB(cudaEventCreate(&h->ev0)); CUB(cudaEventCreate(&h->ev1));
+  CU(h->stream.create());
+  CU(h->ev0.create()); CU(h->ev1.create());
   h->stride = plane_stride(h->count);
-  const size_t inbox_bytes = (size_t)3 * h->R * h->stride * sizeof(u32);
-  CUB(cudaMalloc(&h->d_rec, (size_t)h->R * h->stride * 32));
-  CUB(cudaMemset(h->d_rec, 0, (size_t)h->R * h->stride * 32));
-  CUB(cudaMalloc(&h->d_qword, (size_t)h->R * h->stride * 4));
-  CUB(cudaMemset(h->d_qword, 0, (size_t)h->R * h->stride * 4));
-  CUB(cudaMalloc(&h->d_inbox[0], inbox_bytes)); CUB(cudaMalloc(&h->d_inbox[1], inbox_bytes));
-  CUB(cudaMalloc(&h->d_node, (size_t)h->stride * 8));
-  CUB(cudaMemset(h->d_node, 0, (size_t)h->stride * 8));
   h->n_tiles = h->stride >> TILE_SHIFT;
-  CUB(cudaMalloc(&h->d_busy, h->stride));
-  CUB(cudaMalloc(&h->d_watch, (size_t)h->stride * 2));
-  CUB(cudaMemset(h->d_watch, 0, (size_t)h->stride * 2));
-  CUB(cudaMalloc(&h->d_hot[0], h->n_tiles)); CUB(cudaMalloc(&h->d_hot[1], h->n_tiles));
-  CUB(cudaMalloc(&h->d_hot_static, h->n_tiles)); CUB(cudaMalloc(&h->d_tile_due, (size_t)h->n_tiles * sizeof(u32))); CUB(cudaMalloc(&h->d_node_due, (size_t)h->stride * sizeof(u32))); CUB(cudaMalloc(&h->d_sched, SCHED_WORDS * sizeof(u32)));
-  CUB(cudaMemset(h->d_hot_static, 0, h->n_tiles));
-  if (h->R > 1 && cfg->world_size <= 1) CUB(cudaMalloc(&h->d_carry, (size_t)h->stride * sizeof(u32)));
-  CUB(cudaHostAlloc(&h->pin_overflow, sizeof(u32), cudaHostAllocMapped));
-  CUB(cudaHostGetDevicePointer(&h->d_overflow, h->pin_overflow, 0));
-  *h->pin_overflow = 0;
-  CUB(cudaMalloc(&h->d_subj, MAX_SLOTS * 4)); CUB(cudaMalloc(&h->d_scratch, 64 * 8));
-  CUB(cudaMalloc(&h->d_stage, (size_t)h->count * 8));
-  CUB(cudaMalloc(&h->d_runctl, 2 * sizeof(u32)));
-  CUB(cudaMemset(h->d_runctl, 0, 2 * sizeof(u32)));
-  CUB(cudaHostAlloc(&h->pin_ctl, 4 * sizeof(u32), cudaHostAllocMapped));
-  CUB(cudaHostGetDevicePointer(&h->d_pin_ctl, h->pin_ctl, 0));
-  h->pin_ctl[0] = h->pin_ctl[1] = h->pin_ctl[2] = h->pin_ctl[3] = 0;
-  CUB(cudaMemcpy(h->d_subj, h->subj.data(), h->R * 4, cudaMemcpyHostToDevice));
+  const size_t planes = (size_t)h->R * h->stride;
+  CU(h->d_rec.alloc(2 * planes)); CU(h->d_rec.fill(0, h->stream));
+  CU(h->d_qword.alloc(planes));
+  CU(h->d_inbox[0].alloc(3 * planes)); CU(h->d_inbox[1].alloc(3 * planes));
+  CU(h->d_node.alloc(h->stride)); CU(h->d_node.fill(0, h->stream));
+  CU(h->d_busy.alloc(h->stride));
+  CU(h->d_watch.alloc(h->stride)); CU(h->d_watch.fill(0, h->stream));
+  CU(h->d_hot[0].alloc(h->n_tiles)); CU(h->d_hot[1].alloc(h->n_tiles));
+  CU(h->d_hot_static.alloc(h->n_tiles)); CU(h->d_hot_static.fill(0, h->stream));
+  CU(h->d_tile_due.alloc(h->n_tiles)); CU(h->d_node_due.alloc(h->stride)); CU(h->d_sched.alloc(SCHED_WORDS));
+  if (h->R > 1 && cfg->world_size <= 1) CU(h->d_carry.alloc(h->stride));
+  CU(h->pin_overflow.create(1)); CU(cudaHostGetDevicePointer(&h->d_overflow, h->pin_overflow, 0));
+  CU(h->d_subj.alloc(MAX_SLOTS)); CU(h->d_scratch.alloc(64));
+  CU(h->d_stage.alloc(h->count));
+  CU(h->d_runctl.alloc(2));
+  CU(h->pin_ctl.create(4)); CU(cudaHostGetDevicePointer(&h->d_pin_ctl, h->pin_ctl, 0));
+  CU(cudaMemcpy(h->d_subj, h->subj.data(), h->R * 4, cudaMemcpyHostToDevice));
   h->sw = read_switches();
   cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, dev);
   if (h->sms <= 0) h->sms = 132;
@@ -952,40 +876,30 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   }
   if (cfg->world_size > 1) {
     // receive windows: one segment per peer; expected entries per tick and pair ≈ shard · fanout · R · kinds / world
-    if (cfg->world_size > 8) return bail(fail(SERFSIM_E_INVAL, "world_size > 8"));
+    if (cfg->world_size > 8) return fail(SERFSIM_E_INVAL, "world_size > 8");
     // … plus what a warp of the tick kernel (TILE threads) can leave unfilled in a peer's window: its reservation ahead and a partial block
     const double pad = (double)std::max(h->grid, h->grid_sv) * (TILE / 32) * (XW_RESERVE_MAX + XW_FLUSH);   // (the single-view kernel of a multi-slot run has the larger grid)
     double cap = (double)h->shard_size * cfg->fanout * h->R * 3.0 * h->sw.win_factor / cfg->world_size + 4096.0 + pad;
     h->win_cap = (u32)std::min(cap, 4.0e9);
     h->win_cap_base = h->win_cap;
     for (int par = 0; par < 2; ++par) {
-      CUB(cudaMalloc(&h->d_win_data[par], (size_t)cfg->world_size * h->win_cap * 8));
-      CUB(cudaMemset(h->d_win_data[par], 0, (size_t)cfg->world_size * h->win_cap * 8));      // windows read as zeros wherever nothing was written
-      CUB(cudaMalloc(&h->d_peer_data[par], sizeof(u64*) * 8));
+      CU(h->d_win_data[par].alloc((size_t)cfg->world_size * h->win_cap));
+      CU(h->d_win_data[par].fill(0, h->stream));      // windows read as zeros wherever nothing was written
+      CU(h->d_peer_data[par].alloc(8));
     }
-    CUB(cudaMalloc(&h->d_ctrl, CTRL_BYTES));
-    CUB(cudaMemset(h->d_ctrl, 0, CTRL_BYTES));
-    CUB(cudaMalloc(&h->d_send_count, 8 * sizeof(u32)));
-    CUB(cudaMemset(h->d_send_count, 0, 8 * sizeof(u32)));
-    CUB(cudaMalloc(&h->d_peer_ctrl, sizeof(u32*) * 8));
-    CUB(cudaMalloc(&h->d_anomaly, h->stride)); CUB(cudaMemset(h->d_anomaly, 0, h->stride));   // byzantine sender flags: peers' drain kernels raise them
-    CUB(cudaMalloc(&h->d_byz_totals, 4 * 8)); CUB(cudaMemset(h->d_byz_totals, 0, 4 * 8));
-    CUB(cudaMalloc(&h->d_peer_anomaly, sizeof(void*) * 8));
-    if (cfg->push_pull_interval_ticks > 0) {      // the snapshots partners on other GPUs read: allocated now so that they can be exported
-      CUB(cudaMalloc(&h->d_snap_rec, (size_t)h->R * h->stride * 32));
-      CUB(cudaMalloc(&h->d_snap_node, (size_t)h->stride * 8));
-      CUB(cudaMalloc(&h->d_peer_snap_rec, sizeof(void*) * 8));
-      CUB(cudaMalloc(&h->d_peer_snap_node, sizeof(void*) * 8));
-    }
+    CU(h->d_ctrl.alloc(CTRL_BYTES / sizeof(u32))); CU(h->d_ctrl.fill(0, h->stream));
+    CU(h->d_send_count.alloc(8));
+    CU(h->d_peer_ctrl.alloc(8));
+    serfsim::Injectors b; CU(b.anomaly.alloc(h->stride)); CU(b.totals.alloc(4)); h->byz = std::move(b);   // peers' drain kernels raise the flags
+    CU(h->d_peer_anomaly.alloc(8));
   }
-  {
-    int rc = ensure_trace(h, 1024);
-    if (rc) return bail(rc);
-    rc = do_reset(h, cfg->seed);
-    if (rc) return bail(rc);
+  if (cfg->push_pull_interval_ticks > 0) {         // push-pull rounds' snapshots (sharded runs export them, so all are allocated here)
+    CU(h->d_snap_rec.alloc(h->d_rec.size())); CU(h->d_snap_node.alloc(h->d_node.size()));
+    if (cfg->world_size > 1) { CU(h->d_peer_snap_rec.alloc(8)); CU(h->d_peer_snap_node.alloc(8)); }
   }
-#undef CUB
-  *out = h;
+  if (int rc = ensure_trace(h.get(), 1024)) return rc;
+  if (int rc = do_reset(h.get(), cfg->seed)) return rc;
+  *out = h.release();
   return 0;
 }
 
@@ -1003,7 +917,6 @@ void serfsim_destroy(serfsim_t* h) {
     }
     fprintf(stderr, "rank %d: tick kernels %.3f ms, publish+drain %.3f ms over %zu ticks\n", h->cfg.rank, a, b, n);
   }
-  free_all(h);
   delete h;
 }
 
@@ -1030,12 +943,13 @@ int serfsim_set_topology_csr(serfsim_t* h, const uint64_t* row_ptr, const uint32
     h->max_tile_edges = std::max(h->max_tile_edges, hi - lo);
   }
   for (u64 i = 0; i < ne; ++i) if (col_idx[e0 + i] >= h->N) return fail(SERFSIM_E_INVAL, "col_idx out of range");
-  cudaFree(h->d_rowptr); cudaFree(h->d_col); h->d_rowptr = nullptr; h->d_col = nullptr;
-  CU(cudaMalloc(&h->d_rowptr, rp.size() * 4));
-  CU(cudaMalloc(&h->d_col, (ne + 8) * 4));
-  CU(cudaMemset(h->d_col, 0, (ne + 8) * 4));
-  CU(cudaMemcpy(h->d_rowptr, rp.data(), rp.size() * 4, cudaMemcpyHostToDevice));
-  if (ne) CU(cudaMemcpy(h->d_col, col_idx + e0, ne * 4, cudaMemcpyHostToDevice));
+  DevArray<u32> d_rowptr, d_col;                  // installed together once both hold the new topology
+  CU(d_rowptr.alloc(rp.size()));
+  CU(d_col.alloc(ne + 8));
+  CU(cudaMemset(d_col, 0, d_col.bytes()));
+  CU(cudaMemcpy(d_rowptr, rp.data(), d_rowptr.bytes(), cudaMemcpyHostToDevice));
+  if (ne) CU(cudaMemcpy(d_col, col_idx + e0, ne * 4, cudaMemcpyHostToDevice));
+  h->d_rowptr = std::move(d_rowptr); h->d_col = std::move(d_col);
   // TMA pipeline (single-slot runs): a stage holds the largest tile's CSR span if that is at most 48 KB
   h->stage_col_bytes = 0;
   {
@@ -1060,9 +974,7 @@ int serfsim_set_subjects(serfsim_t* h, const uint32_t* subjects) {
   CU(cudaMemcpy(h->d_subj, h->subj.data(), h->R * 4, cudaMemcpyHostToDevice));
   h->watch_dirty = true;
   // tick 0 with a clean state: re-derive the watchers' busy bits / hot tiles for the new subjects
-  CU(cudaMemsetAsync(h->d_busy, 0, h->stride, h->stream));
-  CU(cudaMemsetAsync(h->d_hot[0], 0, h->n_tiles, h->stream));
-  CU(cudaMemsetAsync(h->d_hot[1], 0, h->n_tiles, h->stream));
+  CU(h->d_busy.fill(0, h->stream)); CU(h->d_hot[0].fill(0, h->stream)); CU(h->d_hot[1].fill(0, h->stream));
   return refresh_watchers(h);
 }
 
@@ -1215,39 +1127,42 @@ int serfsim_ml_state(serfsim_t* h, uint32_t slot, uint8_t* out) { return getter(
 int serfsim_results_async(serfsim_t* h, uint32_t slot, uint8_t* status, uint32_t* status_ltime, uint32_t* lamport) {
   if (!h) return fail(SERFSIM_E_INVAL, "null handle");
   if (slot >= h->R) return fail(SERFSIM_E_INVAL, "slot out of range");
-  if (!h->copy_stream) { CU(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking)); CU(cudaEventCreate(&h->ev_extracted)); }
-  serfsim::ResBuf& b = h->res[h->res_next++ & 3u];
   const size_t n = h->count, n4 = ((n * 4 + 255) / 256) * 256;
-  if (!b.d) { CU(cudaMalloc(&b.d, 2 * n4 + n)); CU(cudaEventCreate(&b.copied)); }
+  if (!h->rb) {
+    serfsim::ReadBack r;
+    CU(r.copy_stream.create()); CU(r.extracted.create());
+    for (serfsim::ResBuf& b : r.res) { CU(b.d.alloc(2 * n4 + n)); CU(b.copied.create()); }
+    h->rb = std::move(r);
+  }
+  serfsim::ReadBack& rb = *h->rb;
+  serfsim::ResBuf& b = rb.res[rb.next++ & 3u];
   if (b.used) CU(cudaStreamWaitEvent(h->stream, b.copied, 0));            // the copy that last read this staging buffer has finished
   if (status_ltime) launch_extract(h->d_rec, h->d_node, h->count, h->stride, slot, EXTRACT_STATUS_LTIME32, b.d, h->stream);
   if (lamport) launch_extract(h->d_rec, h->d_node, h->count, h->stride, slot, EXTRACT_CLOCK32, b.d + n4, h->stream);
   if (status) launch_extract(h->d_rec, h->d_node, h->count, h->stride, slot, EXTRACT_STATUS, b.d + 2 * n4, h->stream);
-  CU(cudaEventRecord(h->ev_extracted, h->stream));
-  CU(cudaStreamWaitEvent(h->copy_stream, h->ev_extracted, 0));
-  if (status_ltime) CU(cudaMemcpyAsync(status_ltime, b.d, n * 4, cudaMemcpyDeviceToHost, h->copy_stream));
-  if (lamport) CU(cudaMemcpyAsync(lamport, b.d + n4, n * 4, cudaMemcpyDeviceToHost, h->copy_stream));
-  if (status) CU(cudaMemcpyAsync(status, b.d + 2 * n4, n, cudaMemcpyDeviceToHost, h->copy_stream));
-  CU(cudaEventRecord(b.copied, h->copy_stream));
+  CU(cudaEventRecord(rb.extracted, h->stream));
+  CU(cudaStreamWaitEvent(rb.copy_stream, rb.extracted, 0));
+  if (status_ltime) CU(cudaMemcpyAsync(status_ltime, b.d, n * 4, cudaMemcpyDeviceToHost, rb.copy_stream));
+  if (lamport) CU(cudaMemcpyAsync(lamport, b.d + n4, n * 4, cudaMemcpyDeviceToHost, rb.copy_stream));
+  if (status) CU(cudaMemcpyAsync(status, b.d + 2 * n4, n, cudaMemcpyDeviceToHost, rb.copy_stream));
+  CU(cudaEventRecord(b.copied, rb.copy_stream));
   b.used = true;
   return 0;
 }
 int serfsim_results_wait(serfsim_t* h) {
   if (!h) return fail(SERFSIM_E_INVAL, "null handle");
-  if (h->copy_stream) CU(cudaStreamSynchronize(h->copy_stream));
+  if (h->rb) CU(cudaStreamSynchronize(h->rb->copy_stream));
   return 0;
 }
 
 int serfsim_records(serfsim_t* h, uint32_t slot, void* out) {
   if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
   if (slot >= h->R) return fail(SERFSIM_E_INVAL, "slot out of range");
-  uint4* tmp = nullptr;                          // merged image: record | transmit budgets of the queue word
-  CU(cudaMalloc(&tmp, (size_t)h->count * 32));
+  DevArray<uint4> tmp;                           // merged image: record | transmit budgets of the queue word
+  CU(tmp.alloc(2 * (size_t)h->count));
   launch_compose_records(h->d_rec, h->d_qword, h->count, h->stride, slot, tmp, h->stream);
-  cudaError_t e = cudaMemcpyAsync(out, tmp, (size_t)h->count * 32, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(tmp);
-  if (e != cudaSuccess) return fail(SERFSIM_E_CUDA, cudaGetErrorString(e));
+  CU(cudaMemcpyAsync(out, tmp, tmp.bytes(), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
@@ -1265,7 +1180,7 @@ int serfsim_state_hash(serfsim_t* h, uint64_t* out) {
   if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
   CU(cudaMemsetAsync(h->d_scratch, 0, 4 * 8, h->stream));
   launch_state_hash(h->d_rec, h->d_qword, h->d_node, h->count, h->stride, h->first, h->N, h->R, h->d_scratch, h->stream);
-  if (h->ue_table.n) launch_ue_summary(h->d_ue_state, h->count, h->first, h->N, h->R, h->ue_table.n, h->d_scratch + 1, h->stream);
+  if (h->ue_table.n) launch_ue_summary(h->ue->state, h->count, h->first, h->N, h->R, h->ue_table.n, h->d_scratch + 1, h->stream);
   u64 parts[4] = {0, 0, 0, 0};
   CU(cudaMemcpyAsync(parts, h->d_scratch, 4 * 8, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -1308,18 +1223,15 @@ int serfsim_set_byzantine(serfsim_t* h, uint32_t n, const uint32_t* ids, uint32_
   for (u32 i = 0; i < n; ++i) if (v[i] >= h->N || (i && v[i] == v[i - 1])) return fail(SERFSIM_E_INVAL, "byzantine ids must be distinct node ids");
   std::vector<u32> mine;                           // every rank is given the global list and keeps the injectors of its shard
   for (u32 id : v) if (id - h->first < h->count) mine.push_back(id);
-  cudaFree(h->d_byz_ids); h->d_byz_ids = nullptr;
-  h->byz_n = 0; h->byz_delta = delta; h->byz_on = n != 0;
-  if (n) {
-    if (!h->d_anomaly) { CU(cudaMalloc(&h->d_anomaly, h->stride)); CU(cudaMalloc(&h->d_byz_totals, 4 * 8)); }
-    if (!mine.empty()) {
-      CU(cudaMalloc(&h->d_byz_ids, mine.size() * 4));
-      CU(cudaMemcpy(h->d_byz_ids, mine.data(), mine.size() * 4, cudaMemcpyHostToDevice));
-    }
-    CU(cudaMemset(h->d_anomaly, 0, h->stride));
-    CU(cudaMemset(h->d_byz_totals, 0, 4 * 8));
-    h->byz_n = (u32)mine.size();
+  DevArray<u32> d_ids;
+  if (!mine.empty()) {
+    CU(d_ids.alloc(mine.size()));
+    CU(cudaMemcpy(d_ids, mine.data(), d_ids.bytes(), cudaMemcpyHostToDevice));
   }
+  if (n && !h->byz) { serfsim::Injectors b; CU(b.anomaly.alloc(h->stride)); CU(b.totals.alloc(4)); h->byz = std::move(b); }
+  if (h->byz) h->byz->ids = std::move(d_ids);
+  h->byz_n = (u32)mine.size(); h->byz_delta = delta; h->byz_on = n != 0;
+  if (n) { CU(cudaMemset(h->byz->anomaly, 0, h->byz->anomaly.bytes())); CU(cudaMemset(h->byz->totals, 0, h->byz->totals.bytes())); }
   return 0;
 }
 
@@ -1331,7 +1243,7 @@ int serfsim_anomaly_flags(serfsim_t* h, uint8_t* out) {
     if (!h->barrier) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
     h->barrier(h->comm_user);
   }
-  CU(cudaMemcpy(out, h->d_anomaly, h->count, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(out, h->byz->anomaly, h->count, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1344,9 +1256,9 @@ int serfsim_byzantine_stats(serfsim_t* h, serfsim_byz_stats_t* o) {
     if (!h->barrier || !h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
     h->barrier(h->comm_user);                      // see serfsim_anomaly_flags
   }
-  CU(cudaMemcpy(t, h->d_byz_totals, 4 * 8, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(t, h->byz->totals, h->byz->totals.bytes(), cudaMemcpyDeviceToHost));
   std::vector<u8> flags(h->count);
-  CU(cudaMemcpy(flags.data(), h->d_anomaly, h->count, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(flags.data(), h->byz->anomaly, h->count, cudaMemcpyDeviceToHost));
   u64 v[3] = {t[0], t[1], 0};
   for (u8 f : flags) v[2] += f ? 1 : 0;
   if (h->cfg.world_size > 1) h->allreduce(h->comm_user, v, 3);
@@ -1367,25 +1279,18 @@ int serfsim_set_user_events(serfsim_t* h, uint32_t n_events, const uint32_t* con
     const u32 want = (u32)std::min(cap, 4.0e9);
     if (want != h->win_cap) {
       if (h->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs call it before serfsim_comm_export / serfsim_comm_connect (it resizes the receive windows)");
-      for (int par = 0; par < 2; ++par) {
-        cudaFree(h->d_win_data[par]); h->d_win_data[par] = nullptr;
-        CU(cudaMalloc(&h->d_win_data[par], (size_t)h->cfg.world_size * want * 8));
-        CU(cudaMemset(h->d_win_data[par], 0, (size_t)h->cfg.world_size * want * 8));
-      }
+      for (int par = 0; par < 2; ++par) { CU(h->d_win_data[par].alloc((size_t)h->cfg.world_size * want)); CU(h->d_win_data[par].fill(0, h->stream)); }
       h->win_cap = want;
     }
   }
-  if (n_events && !h->d_ue_state) {
-    CU(cudaMalloc(&h->d_ue_state, (size_t)h->stride * 16));
-    CU(cudaMalloc(&h->d_ue_inbox[0], (size_t)h->stride * 4));
-    CU(cudaMalloc(&h->d_ue_inbox[1], (size_t)h->stride * 4));
-    CU(cudaMalloc(&h->d_ue_ltime, MAX_UEVENTS * 4));
-    CU(cudaMalloc(&h->d_ue_totals, 8 * 8));
-  }
-  if (n_events && h->cfg.push_pull_interval_ticks > 0 && !h->d_ue_snap) {
-    if (h->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs with push-pull rounds call it before serfsim_comm_export (the event snapshot is exported)");
-    CU(cudaMalloc(&h->d_ue_snap, (size_t)h->stride * 16));
-    CU(cudaMalloc(&h->d_peer_ue_snap, sizeof(void*) * 8));
+  if (n_events && !h->ue) {
+    const bool pp = h->cfg.push_pull_interval_ticks > 0;
+    if (pp && h->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs with push-pull rounds call it before serfsim_comm_export (the event snapshot is exported)");
+    serfsim::UserEvents u;
+    CU(u.state.alloc(h->stride)); CU(u.inbox[0].alloc(h->stride)); CU(u.inbox[1].alloc(h->stride));
+    CU(u.ltime.alloc(MAX_UEVENTS)); CU(u.totals.alloc(8));
+    if (pp) { CU(u.snap.alloc(h->stride)); CU(u.peer_snap.alloc(8)); }
+    h->ue = std::move(u);
   }
   h->ue_table = UeTable{};
   h->ue_table.n = n_events;
@@ -1439,7 +1344,7 @@ int serfsim_set_user_event_content(serfsim_t* h, uint32_t n, const uint8_t* cons
   }
   t.off[n] = (u32)buf.size();
   t.n = n;
-  if (!h->d_ue_entries) CU(cudaMalloc(&h->d_ue_entries, wire::UE_TABLE_MAX * wire::UE_ENTRY_MAX));
+  if (!h->d_ue_entries) CU(h->d_ue_entries.alloc(wire::UE_TABLE_MAX * wire::UE_ENTRY_MAX));
   CU(cudaStreamSynchronize(h->stream));             // no wire kernel is still reading the old table
   CU(cudaMemcpy(h->d_ue_entries, buf.data(), buf.size(), cudaMemcpyHostToDevice));
   t.entries = h->d_ue_entries;
@@ -1450,7 +1355,7 @@ int serfsim_set_user_event_content(serfsim_t* h, uint32_t n, const uint8_t* cons
 int serfsim_event_time(serfsim_t* h, uint64_t* out) {
   if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
   if (!h->ue_table.n) return fail(SERFSIM_E_INVAL, "user events are off (serfsim_set_user_events)");
-  launch_ue_extract(h->d_ue_state, h->count, 0, 0, h->d_stage, h->stream);
+  launch_ue_extract(h->ue->state, h->count, 0, 0, h->d_stage, h->stream);
   CU(cudaMemcpyAsync(out, h->d_stage, (size_t)h->count * 8, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   return 0;
@@ -1459,7 +1364,7 @@ int serfsim_event_time(serfsim_t* h, uint64_t* out) {
 int serfsim_user_event_seen(serfsim_t* h, uint32_t event, uint8_t* out) {
   if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
   if (event >= h->ue_table.n) return fail(SERFSIM_E_INVAL, "user event index out of range");
-  launch_ue_extract(h->d_ue_state, h->count, 1, event, h->d_stage, h->stream);
+  launch_ue_extract(h->ue->state, h->count, 1, event, h->d_stage, h->stream);
   CU(cudaMemcpyAsync(out, h->d_stage, (size_t)h->count, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   return 0;
@@ -1480,7 +1385,7 @@ int serfsim_user_event_records(serfsim_t* h, void* out) {
   if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
   if (!h->ue_table.n) return fail(SERFSIM_E_INVAL, "user events are off (serfsim_set_user_events)");
   CU(cudaStreamSynchronize(h->stream));
-  CU(cudaMemcpy(out, h->d_ue_state, (size_t)h->count * 16, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(out, h->ue->state, (size_t)h->count * 16, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1490,9 +1395,9 @@ int serfsim_user_event_stats(serfsim_t* h, serfsim_uevent_stats_t* o) {
   if (!h->ue_table.n) return fail(SERFSIM_E_INVAL, "user events are off (serfsim_set_user_events)");
   u64 tot[8] = {0}, sum[3] = {0, 0, 0};
   CU(cudaMemsetAsync(h->d_scratch, 0, 3 * 8, h->stream));
-  launch_ue_summary(h->d_ue_state, h->count, h->first, h->N, h->R, h->ue_table.n, h->d_scratch, h->stream);
+  launch_ue_summary(h->ue->state, h->count, h->first, h->N, h->R, h->ue_table.n, h->d_scratch, h->stream);
   CU(cudaMemcpyAsync(sum, h->d_scratch, 3 * 8, cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaMemcpyAsync(tot, h->d_ue_totals, 8 * 8, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaMemcpyAsync(tot, h->ue->totals, h->ue->totals.bytes(), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   u64 v[6] = {tot[0], tot[1], tot[2], tot[3], tot[4], sum[0]};
   if (h->cfg.world_size > 1) {                      // counters are sums over shards; event_time (a maximum) stays shard-local
@@ -1553,8 +1458,8 @@ int serfsim_comm_export(serfsim_t* h, void* blob) {
   comm_blob b{};
   for (int par = 0; par < 2; ++par) CU(cudaIpcGetMemHandle(&b.data[par], h->d_win_data[par]));
   CU(cudaIpcGetMemHandle(&b.ctrl, h->d_ctrl));
-  CU(cudaIpcGetMemHandle(&b.anomaly, h->d_anomaly));
-  if (h->d_ue_snap) { CU(cudaIpcGetMemHandle(&b.ue_snap, h->d_ue_snap)); b.has_ue_snap = 1; }
+  CU(cudaIpcGetMemHandle(&b.anomaly, h->byz->anomaly));
+  if (h->ue && h->ue->snap) { CU(cudaIpcGetMemHandle(&b.ue_snap, h->ue->snap)); b.has_ue_snap = 1; }
   b.win_cap = h->win_cap; b.rank = (u32)h->cfg.rank;
 #ifndef SERFSIM_EMU
   { int dev = 0; cudaDeviceProp pr{}; CU(cudaGetDevice(&dev)); CU(cudaGetDeviceProperties(&pr, dev)); memcpy(b.dev_uuid, pr.uuid.bytes, 16); }
@@ -1579,6 +1484,7 @@ int serfsim_comm_connect(serfsim_t* h, const void* blobs) {
   std::vector<const u64*> psn(8, nullptr);
   std::vector<u8*> pan(8, nullptr);
   std::vector<const uint4*> pus(8, nullptr);
+  const uint4* ue_snap = h->ue ? h->ue->snap.get() : nullptr;
   for (int r = 0; r < W; ++r) {
     if (bs[r].rank != (u32)r || bs[r].win_cap != h->win_cap) return fail(SERFSIM_E_COMM, "blob order / window size mismatch");
 #ifndef SERFSIM_EMU
@@ -1586,8 +1492,8 @@ int serfsim_comm_connect(serfsim_t* h, const void* blobs) {
     for (int r2 = 0; r2 < r; ++r2) if (!h->loopback && memcmp(bs[r].dev_uuid, bs[r2].dev_uuid, 16) == 0) return fail(SERFSIM_E_COMM, "two ranks share one GPU (one process per GPU is required)");
 #endif
     if ((bs[r].has_snap != 0) != (h->d_snap_rec != nullptr)) return fail(SERFSIM_E_COMM, "push_pull_interval_ticks differs between ranks");
-    if (r == h->cfg.rank) { pd[0][r] = h->d_win_data[0]; pd[1][r] = h->d_win_data[1]; pc[r] = h->d_ctrl; psr[r] = h->d_snap_rec; psn[r] = h->d_snap_node; pan[r] = h->d_anomaly; pus[r] = h->d_ue_snap; continue; }
-    if ((bs[r].has_ue_snap != 0) != (h->d_ue_snap != nullptr)) return fail(SERFSIM_E_COMM, "user events / push-pull configuration differs between ranks");
+    if (r == h->cfg.rank) { pd[0][r] = h->d_win_data[0]; pd[1][r] = h->d_win_data[1]; pc[r] = h->d_ctrl; psr[r] = h->d_snap_rec; psn[r] = h->d_snap_node; pan[r] = h->byz->anomaly; pus[r] = ue_snap; continue; }
+    if ((bs[r].has_ue_snap != 0) != (ue_snap != nullptr)) return fail(SERFSIM_E_COMM, "user events / push-pull configuration differs between ranks");
     int rc = bs[r].has_ue_snap ? ipc_open(h, bs[r].ue_snap, "event snapshot", &pus[r]) : 0;
     if (!rc) rc = ipc_open(h, bs[r].anomaly, "flags", &pan[r]);
     if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_rec, "snapshot", &psr[r]);
@@ -1596,13 +1502,13 @@ int serfsim_comm_connect(serfsim_t* h, const void* blobs) {
     if (!rc) rc = ipc_open(h, bs[r].ctrl, "ctrl", &pc[r]);
     if (rc) return rc;
   }
-  for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), sizeof(u64*) * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), sizeof(u32*) * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_anomaly, pan.data(), sizeof(void*) * 8, cudaMemcpyHostToDevice));
-  if (h->d_ue_snap) CU(cudaMemcpy(h->d_peer_ue_snap, pus.data(), sizeof(void*) * 8, cudaMemcpyHostToDevice));
+  for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), h->d_peer_data[par].bytes(), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), h->d_peer_ctrl.bytes(), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(h->d_peer_anomaly, pan.data(), h->d_peer_anomaly.bytes(), cudaMemcpyHostToDevice));
+  if (ue_snap) CU(cudaMemcpy(h->ue->peer_snap, pus.data(), h->ue->peer_snap.bytes(), cudaMemcpyHostToDevice));
   if (h->d_snap_rec) {
-    CU(cudaMemcpy(h->d_peer_snap_rec, psr.data(), sizeof(void*) * 8, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(h->d_peer_snap_node, psn.data(), sizeof(void*) * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(h->d_peer_snap_rec, psr.data(), h->d_peer_snap_rec.bytes(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(h->d_peer_snap_node, psn.data(), h->d_peer_snap_node.bytes(), cudaMemcpyHostToDevice));
   }
   h->barrier(h->comm_user);          // every rank has mapped every window before the first tick writes into one
   h->connected = true;
@@ -1620,12 +1526,12 @@ int serfsim_comm_loopback(serfsim_t* h) {
   std::vector<std::vector<u64*>> pd(2, std::vector<u64*>(8, nullptr));
   std::vector<u8*> pan(8, nullptr);
   for (int r = 0; r < W; ++r) {
-    pc[r] = h->d_ctrl; pan[r] = h->d_anomaly;
+    pc[r] = h->d_ctrl; pan[r] = h->byz->anomaly;
     for (int par = 0; par < 2; ++par) pd[par][r] = h->d_win_data[par] + (size_t)r * h->win_cap;
   }
-  for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), sizeof(u64*) * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), sizeof(u32*) * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_anomaly, pan.data(), sizeof(void*) * 8, cudaMemcpyHostToDevice));
+  for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), h->d_peer_data[par].bytes(), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), h->d_peer_ctrl.bytes(), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(h->d_peer_anomaly, pan.data(), h->d_peer_anomaly.bytes(), cudaMemcpyHostToDevice));
   h->barrier = [](void*) {};
   h->allreduce = [](void*, uint64_t*, uint32_t) {};
   h->connected = true; h->loopback = true;

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/serfsim.h"
+#include "owned.cuh"
 #include "tick_kernel.cuh"
 #include "wire.cuh"
 
@@ -21,7 +22,6 @@ struct serfsim;                                   // serfsim.cu
 namespace sfs {
 struct WireView { const uint4* rec; const u32* qword; const u64* node_state; const uint4* ue_state; const u32* subj; u32 n_local, stride, R; cudaStream_t stream; wire::UeWire ue; };
 int serfsim_wire_view(const serfsim* h, WireView* out);          // serfsim.cu: the device arrays a batch encode reads
-int serfsim_fail(int code, const char* msg);
 }
 
 namespace {
@@ -431,22 +431,20 @@ int serfsim_wire_local_state_range(serfsim_t* h, uint32_t first, uint32_t count,
   if (rc) return rc;
   if (first > v.n_local || count > v.n_local - first) return serfsim_fail(SERFSIM_E_INVAL, "wire: node range outside the shard");
   const u32 n = count;
-  u64 *d_len = nullptr, *d_off = nullptr; u8* d_out = nullptr;
-  auto cleanup = [&]() { cudaFree(d_len); cudaFree(d_off); cudaFree(d_out); };
-#define CW(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return serfsim_fail(SERFSIM_E_CUDA, cudaGetErrorString(e_)); } } while (0)
-  CW(cudaMalloc(&d_len, (size_t)n * 8 + 8)); CW(cudaMalloc(&d_off, ((size_t)n + 1) * 8));
-  if (n) SFS_LAUNCH((n + 255) / 256, 256, 0, v.stream, pp_len_kernel)(v, first, n, d_len);
-  SFS_LAUNCH(1, 1024, 0, v.stream, pp_scan_kernel)(d_len, d_off, n);
-  CW(cudaMemcpyAsync(offsets, d_off, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaStreamSynchronize(v.stream));
+  DevArray<u64> d_len, d_off;
+  DevArray<u8> d_out;
+  CU(d_len.alloc((size_t)n + 1)); CU(d_off.alloc((size_t)n + 1));
+  if (n) SFS_LAUNCH((n + 255) / 256, 256, 0, v.stream, pp_len_kernel)(v, first, n, d_len.get());
+  SFS_LAUNCH(1, 1024, 0, v.stream, pp_scan_kernel)(d_len.get(), d_off.get(), n);
+  CU(cudaMemcpyAsync(offsets, d_off, d_off.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaStreamSynchronize(v.stream));
   *total = (size_t)offsets[n];
-  if (!out || cap < *total) { cleanup(); return werr(w::E_CAPACITY); }
-  CW(cudaMalloc(&d_out, *total ? *total : 1));
-  if (n) SFS_LAUNCH((n + EMIT_THREADS - 1) / EMIT_THREADS, EMIT_THREADS, 0, v.stream, pp_emit_kernel)(v, first, n, d_off, d_out, (u64)*total);
-  CW(cudaMemcpyAsync(out, d_out, *total, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaStreamSynchronize(v.stream));
-  CW(cudaGetLastError());
-  cleanup();
+  if (!out || cap < *total) return werr(w::E_CAPACITY);
+  CU(d_out.alloc(*total ? *total : 1));
+  if (n) SFS_LAUNCH((n + EMIT_THREADS - 1) / EMIT_THREADS, EMIT_THREADS, 0, v.stream, pp_emit_kernel)(v, first, n, d_off.get(), d_out.get(), (u64)*total);
+  CU(cudaMemcpyAsync(out, d_out, *total, cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaStreamSynchronize(v.stream));
+  CU(cudaGetLastError());
   return 0;
 }
 
@@ -469,23 +467,22 @@ int serfsim_wire_decode_batch(serfsim_t* h, const uint8_t* buf, const uint64_t* 
   if ((rc = check_batch_offsets(offsets, n))) return rc;
   if (!n) return 0;                                          // nothing to decode
   const size_t total = (size_t)offsets[n];
-  u8* d_buf = nullptr; u64 *d_off = nullptr, *d_lt = nullptr, *d_ids = nullptr, *d_sts = nullptr; u32 *d_ns = nullptr, *d_err = nullptr;
-  auto cleanup = [&]() { cudaFree(d_buf); cudaFree(d_off); cudaFree(d_lt); cudaFree(d_ids); cudaFree(d_sts); cudaFree(d_ns); cudaFree(d_err); };
-  CW(cudaMalloc(&d_buf, total ? total : 1)); CW(cudaMalloc(&d_off, ((size_t)n + 1) * 8)); CW(cudaMalloc(&d_lt, (size_t)n * 8 + 8));
-  CW(cudaMalloc(&d_ids, (size_t)n * cap * 8 + 8)); CW(cudaMalloc(&d_sts, (size_t)n * cap * 8 + 8)); CW(cudaMalloc(&d_ns, (size_t)n * 4 + 4)); CW(cudaMalloc(&d_err, (size_t)n * 4 + 4));
-  CW(cudaMemcpyAsync(d_buf, buf, total, cudaMemcpyHostToDevice, v.stream));
-  CW(cudaMemcpyAsync(d_off, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, v.stream));
-  if (n) SFS_LAUNCH((n + 127) / 128, 128, 0, v.stream, pp_decode_kernel)(d_buf, d_off, n, cap, d_lt, d_ids, d_sts, d_ns, d_err);
+  DevArray<u8> d_buf;
+  DevArray<u64> d_off, d_lt, d_ids, d_sts;
+  DevArray<u32> d_ns, d_err;
+  CU(d_buf.alloc(total ? total : 1)); CU(d_off.alloc((size_t)n + 1)); CU(d_lt.alloc(n));
+  CU(d_ids.alloc((size_t)n * cap)); CU(d_sts.alloc((size_t)n * cap)); CU(d_ns.alloc(n)); CU(d_err.alloc(n));
+  CU(cudaMemcpyAsync(d_buf, buf, total, cudaMemcpyHostToDevice, v.stream));
+  CU(cudaMemcpyAsync(d_off, offsets, d_off.bytes(), cudaMemcpyHostToDevice, v.stream));
+  SFS_LAUNCH((n + 127) / 128, 128, 0, v.stream, pp_decode_kernel)(d_buf.get(), d_off.get(), n, cap, d_lt.get(), d_ids.get(), d_sts.get(), d_ns.get(), d_err.get());
   std::vector<u32> err(n);
-  CW(cudaMemcpyAsync(ltime, d_lt, (size_t)n * 8, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(ids, d_ids, (size_t)n * cap * 8, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(status_ltimes, d_sts, (size_t)n * cap * 8, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(n_status, d_ns, (size_t)n * 4, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(err.data(), d_err, (size_t)n * 4, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaStreamSynchronize(v.stream));
-  CW(cudaGetLastError());
-  cleanup();
-#undef CW
+  CU(cudaMemcpyAsync(ltime, d_lt, d_lt.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(ids, d_ids, d_ids.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(status_ltimes, d_sts, d_sts.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(n_status, d_ns, d_ns.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(err.data(), d_err, d_err.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaStreamSynchronize(v.stream));
+  CU(cudaGetLastError());
   for (u32 i = 0; i < n; ++i)
     if (err[i] & 0x80000000u) { werr(-(int)(err[i] & 0xffffu)); return serfsim_fail(SERFSIM_E_INVAL, (std::string("wire: message ") + std::to_string(i) + ": " + serfsim_last_error()).c_str()); }
   return 0;
@@ -564,23 +561,21 @@ int serfsim_wire_decode_events_batch(serfsim_t* h, const uint8_t* buf, const uin
   if ((rc = check_batch_offsets(offsets, n))) return rc;
   if (!n) return 0;                                          // nothing to decode
   const size_t total = (size_t)offsets[n];
-  u8* d_buf = nullptr; u64 *d_off = nullptr, *d_ev = nullptr; u32 *d_seen = nullptr, *d_um = nullptr, *d_err = nullptr;
-  auto cleanup = [&]() { cudaFree(d_buf); cudaFree(d_off); cudaFree(d_ev); cudaFree(d_seen); cudaFree(d_um); cudaFree(d_err); };
-#define CW(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return serfsim_fail(SERFSIM_E_CUDA, cudaGetErrorString(e_)); } } while (0)
-  CW(cudaMalloc(&d_buf, total ? total : 1)); CW(cudaMalloc(&d_off, ((size_t)n + 1) * 8)); CW(cudaMalloc(&d_ev, (size_t)n * 8 + 8));
-  CW(cudaMalloc(&d_seen, (size_t)n * 4 + 4)); CW(cudaMalloc(&d_um, (size_t)n * 4 + 4)); CW(cudaMalloc(&d_err, (size_t)n * 4 + 4));
-  CW(cudaMemcpyAsync(d_buf, buf, total, cudaMemcpyHostToDevice, v.stream));
-  CW(cudaMemcpyAsync(d_off, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, v.stream));
-  if (n) SFS_LAUNCH((n + 127) / 128, 128, 0, v.stream, pp_events_decode_kernel)(d_buf, d_off, n, v.ue, d_ev, d_seen, d_um, d_err);
+  DevArray<u8> d_buf;
+  DevArray<u64> d_off, d_ev;
+  DevArray<u32> d_seen, d_um, d_err;
+  CU(d_buf.alloc(total ? total : 1)); CU(d_off.alloc((size_t)n + 1)); CU(d_ev.alloc(n));
+  CU(d_seen.alloc(n)); CU(d_um.alloc(n)); CU(d_err.alloc(n));
+  CU(cudaMemcpyAsync(d_buf, buf, total, cudaMemcpyHostToDevice, v.stream));
+  CU(cudaMemcpyAsync(d_off, offsets, d_off.bytes(), cudaMemcpyHostToDevice, v.stream));
+  SFS_LAUNCH((n + 127) / 128, 128, 0, v.stream, pp_events_decode_kernel)(d_buf.get(), d_off.get(), n, v.ue, d_ev.get(), d_seen.get(), d_um.get(), d_err.get());
   std::vector<u32> err(n);
-  CW(cudaMemcpyAsync(event_ltime, d_ev, (size_t)n * 8, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(seen, d_seen, (size_t)n * 4, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(n_unmatched, d_um, (size_t)n * 4, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaMemcpyAsync(err.data(), d_err, (size_t)n * 4, cudaMemcpyDeviceToHost, v.stream));
-  CW(cudaStreamSynchronize(v.stream));
-  CW(cudaGetLastError());
-  cleanup();
-#undef CW
+  CU(cudaMemcpyAsync(event_ltime, d_ev, d_ev.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(seen, d_seen, d_seen.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(n_unmatched, d_um, d_um.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaMemcpyAsync(err.data(), d_err, d_err.bytes(), cudaMemcpyDeviceToHost, v.stream));
+  CU(cudaStreamSynchronize(v.stream));
+  CU(cudaGetLastError());
   for (u32 i = 0; i < n; ++i)
     if (err[i] & 0x80000000u) { werr(-(int)(err[i] & 0xffffu)); return serfsim_fail(SERFSIM_E_INVAL, (std::string("wire: message ") + std::to_string(i) + ": " + serfsim_last_error()).c_str()); }
   return 0;

@@ -13,6 +13,7 @@
 // the hardware does.  __shared__ becomes `static` (CTAs run one after another).  Atomics are plain read-modify-writes.
 #pragma once
 #include <algorithm>
+#include <atomic>
 #include <cstddef>
 #include <cstdint>
 #include <cstdio>
@@ -55,6 +56,14 @@ unsigned warp_reduce_or(unsigned v);
 unsigned lane_id();
 void polite_wait(unsigned long spins);                          // yields the OS thread; aborts the process after ~120 s of fruitless polling (a peer rank died)
 extern unsigned long probes[32];                              // coverage probes: SFS_PROBE(i) in the kernels, read by tests through emu_probe()
+// Resource accounting for the handle-lifetime tests (emu_live_allocs / emu_fail_alloc_at): device and mapped host allocations,
+// streams, events and IPC mappings alive now, and a countdown to the allocation that is made to fail.  Ranks are threads: atomic.
+extern std::atomic<long> live_allocs, fail_countdown;
+inline bool alloc_fails() {                                   // true for the armed call: the countdown reaches 1 -> 0 here
+  long c = fail_countdown.load();
+  while (c > 0 && !fail_countdown.compare_exchange_weak(c, c - 1)) {}
+  return c == 1;
+}
 
 template <class F>
 struct Bound {
@@ -134,27 +143,38 @@ enum { cudaIpcMemLazyEnablePeerAccess = 1 };
 
 template <class T> inline cudaError_t cudaMalloc(T** p, size_t n) {
   void* q = nullptr;
-  if (posix_memalign(&q, 256, n ? ((n + 255) / 256) * 256 : 256)) return cudaErrorMemoryAllocation;
+  if (emu::alloc_fails() || posix_memalign(&q, 256, n ? ((n + 255) / 256) * 256 : 256)) return cudaErrorMemoryAllocation;
   memset(q, 0xA5, n);                                        // like the device: fresh memory is NOT zero
   *p = (T*)q;
+  emu::live_allocs++;
   return cudaSuccess;
 }
-inline cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
+inline cudaError_t cudaFree(void* p) { if (p) emu::live_allocs--; free(p); return cudaSuccess; }
 template <class T> inline cudaError_t cudaMallocHost(T** p, size_t n) { *p = (T*)malloc(n ? n : 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-inline cudaError_t cudaFreeHost(void* p) { free(p); return cudaSuccess; }
+inline cudaError_t cudaFreeHost(void* p) { if (p) emu::live_allocs--; free(p); return cudaSuccess; }
 constexpr unsigned cudaHostAllocMapped = 2;
-template <class T> inline cudaError_t cudaHostAlloc(T** p, size_t n, unsigned) { *p = (T*)malloc(n ? n : 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+template <class T> inline cudaError_t cudaHostAlloc(T** p, size_t n, unsigned) {
+  if (emu::alloc_fails() || !(*p = (T*)malloc(n ? n : 1))) return cudaErrorMemoryAllocation;
+  emu::live_allocs++;
+  return cudaSuccess;
+}
 template <class T> inline cudaError_t cudaHostGetDevicePointer(T** d, void* h, unsigned) { *d = (T*)h; return cudaSuccess; }
 inline cudaError_t cudaMemset(void* p, int v, size_t n) { memset(p, v, n); return cudaSuccess; }
 inline cudaError_t cudaMemsetAsync(void* p, int v, size_t n, cudaStream_t) { memset(p, v, n); return cudaSuccess; }
 inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { memmove(d, s, n); return cudaSuccess; }
 inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { memmove(d, s, n); return cudaSuccess; }
-inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = (cudaStream_t)malloc(8); return cudaSuccess; }
-inline cudaError_t cudaStreamDestroy(cudaStream_t s) { free(s); return cudaSuccess; }
+inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) {
+  if (emu::alloc_fails()) return cudaErrorMemoryAllocation;
+  *s = (cudaStream_t)malloc(8); emu::live_allocs++; return cudaSuccess;
+}
+inline cudaError_t cudaStreamDestroy(cudaStream_t s) { emu::live_allocs--; free(s); return cudaSuccess; }
 inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 inline cudaError_t cudaStreamSetAttribute(cudaStream_t, cudaStreamAttrID, const cudaStreamAttrValue*) { return cudaSuccess; }
-inline cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = (cudaEvent_t)malloc(8); return cudaSuccess; }
-inline cudaError_t cudaEventDestroy(cudaEvent_t e) { free(e); return cudaSuccess; }
+inline cudaError_t cudaEventCreate(cudaEvent_t* e) {
+  if (emu::alloc_fails()) return cudaErrorMemoryAllocation;
+  *e = (cudaEvent_t)malloc(8); emu::live_allocs++; return cudaSuccess;
+}
+inline cudaError_t cudaEventDestroy(cudaEvent_t e) { emu::live_allocs--; free(e); return cudaSuccess; }
 inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t) { return cudaSuccess; }
 inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
 inline cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned) { return cudaSuccess; }
@@ -176,5 +196,5 @@ inline cudaError_t cudaDeviceSetLimit(cudaLimit, size_t) { return cudaSuccess; }
 template <class F> inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int) { return cudaSuccess; }
 // "IPC" between ranks that are threads of one process: the handle is the pointer itself
 inline cudaError_t cudaIpcGetMemHandle(cudaIpcMemHandle_t* h, void* p) { memset(h, 0, sizeof(*h)); memcpy(h->reserved, &p, sizeof(p)); return cudaSuccess; }
-inline cudaError_t cudaIpcOpenMemHandle(void** out, cudaIpcMemHandle_t h, unsigned) { memcpy(out, h.reserved, sizeof(*out)); return cudaSuccess; }
-inline cudaError_t cudaIpcCloseMemHandle(void*) { return cudaSuccess; }
+inline cudaError_t cudaIpcOpenMemHandle(void** out, cudaIpcMemHandle_t h, unsigned) { memcpy(out, h.reserved, sizeof(*out)); emu::live_allocs++; return cudaSuccess; }
+inline cudaError_t cudaIpcCloseMemHandle(void*) { emu::live_allocs--; return cudaSuccess; }

@@ -46,6 +46,7 @@ namespace emu {
 
 thread_local LaneCtx* cur = nullptr;
 unsigned long probes[32] = {0};
+std::atomic<long> live_allocs{0}, fail_countdown{0};
 
 namespace {
 constexpr int MAX_THREADS = 1024;
@@ -231,3 +232,7 @@ void run_grid(unsigned grid, unsigned block, const std::function<void()>& fn) {
 
 extern "C" __attribute__((visibility("default"))) unsigned long emu_probe(int i) { return emu::probes[i & 31]; }
 extern "C" __attribute__((visibility("default"))) void emu_probe_reset() { for (auto& p : emu::probes) p = 0; }
+// Resources alive now (cuda_runtime.h: live_allocs), and k >= 1: the k-th next allocation, stream or event creation fails with
+// cudaErrorMemoryAllocation (0: none).
+extern "C" __attribute__((visibility("default"))) long emu_live_allocs() { return emu::live_allocs.load(); }
+extern "C" __attribute__((visibility("default"))) void emu_fail_alloc_at(long k) { emu::fail_countdown.store(k); }
