@@ -248,8 +248,8 @@ int serfsim_user_event_stats (serfsim_t* h, serfsim_uevent_stats_t* out);
  * and nothing merged.  Works sharded: every rank passes the GLOBAL id list and keeps the injectors of its shard; an
  * entry bound for another shard is judged by that shard against its own record and the flag is raised in the
  * sender's shard over NVLink.  With push-pull rounds on, the verdict of a tick is taken before that tick's round. */
-/* In sharded runs the three calls below and serfsim_user_event_stats / serfsim_user_event_ltime are COLLECTIVE: every rank
- * makes the same calls in the same order (they use the barrier / all-reduce hooks of serfsim_comm_set_hooks). */
+/* In sharded runs the three calls below, serfsim_user_event_stats / serfsim_user_event_ltime and serfsim_state_hash are COLLECTIVE:
+ * every rank makes the same calls in the same order (they use the barrier / all-reduce hooks of serfsim_comm_set_hooks). */
 int serfsim_set_byzantine  (serfsim_t* h, uint32_t n, const uint32_t* ids /*[n]*/, uint32_t delta);
 int serfsim_anomaly_flags  (serfsim_t* h, uint8_t* out /*[count]*/);
 int serfsim_byzantine_stats(serfsim_t* h, serfsim_byz_stats_t* out);

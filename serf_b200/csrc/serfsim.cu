@@ -39,6 +39,7 @@ thread_local std::string g_err;
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
 struct HostOp { u32 tick, op, node, slot; u64 seq; };
+constexpr int MAX_WORLD = 8;     // ranks of a sharded run
 
 // memberlist retransmit limit: retransmit_mult * ceil(log10(n + 1))  [external crate, restated].  In 64 bits: serfsim_create
 // rejects a product outside 1..255 (the budgets are u8) instead of letting it wrap in u32.
@@ -175,8 +176,6 @@ struct serfsim {
   bool watch_dirty = true;
   DevArray<uint4> d_snap_rec;      // push-pull rounds (allocated by serfsim_create): end-of-tick snapshot of the records …
   DevArray<u64> d_snap_node;       // … and of the node words
-  DevArray<const uint4*> d_peer_snap_rec;   // sharded push-pull: device arrays of every rank's snapshot pointers
-  DevArray<const u64*> d_peer_snap_node;
   DevArray<u8> d_hot[2];                  // [n_tiles] per tick parity
   DevArray<u8> d_hot_static;              // [n_tiles] tiles that hold a watcher (never consumed)
   DevArray<u32> d_node_due;               // [stride] per-node earliest suspicion deadline (tick_kernel.cuh)
@@ -213,7 +212,6 @@ struct serfsim {
   bool byz_on = false;             // any injector anywhere (all ranks agree): changes the convergence rule and the drain kernel
   struct Injectors { DevArray<u8> anomaly; DevArray<u64> totals; DevArray<u32> ids; };
   std::optional<Injectors> byz;
-  DevArray<u8*> d_peer_anomaly;    // sharded runs: device array of every rank's flag array
   // host state
   std::vector<HostOp> ops;         // sorted by (tick, seq)
   std::unordered_set<u64> op_keys; // (tick << 32 | node): at most one operation per node per tick
@@ -233,7 +231,6 @@ struct serfsim {
   DevArray<u32> d_runctl;          // [0] done flag, [1] first quiescent tick
   MappedWords pin_ctl;             // [4] the verdict, written by the gate's leader thread and read once per chunk
   u32* d_pin_ctl = nullptr;        // its device address
-  DevArray<u64> d_grow;            // sharded runs: [trace_cap][8] global trace rows, summed on the device by the drain kernel
   bool gate_on = false;
   u32 gate_first = 0;              // first tick of the current run_until_converged call (it always runs)
   std::vector<u32> launch_log;     // kernels launched per tick since the timing window opened (ticks past the quiescent one do not count)
@@ -248,19 +245,23 @@ struct serfsim {
   int ctas_per_sm = 4;             // resident CTAs per SM the membership kernel's grid is sized for (and its __launch_bounds__ instance)
   int sms = 132;                   // the device's SM count
   Switches sw;                     // run-time switches, read at serfsim_create
-  // multi-GPU
-  DevArray<u64> d_win_data[2];                 // my receive windows [parity][world][win_cap]  (IPC-exported)
-  DevArray<u32> d_ctrl;                        // my control block [parity][counts[8] | flags[8]] (IPC-exported)
-  DevArray<u32> d_send_count;                  // [world] entries written into each peer's window this tick
-  DevArray<u64*> d_peer_data[2];               // device arrays of peer window pointers, per parity
-  DevArray<u32*> d_peer_ctrl;                  // device array of peer control-block pointers
-  u32 xepoch = 0;                              // executed-tick counter of the exchange (never rewinds): stamps and parity
-  u32 win_cap = 0;
-  u32 win_cap_base = 0;                        // capacity sized for the membership entries alone (serfsim_create)
-  bool connected = false;
-  bool loopback = false;                       // serfsim_comm_loopback: profiling aid, the handle exchanges with itself
-  serfsim_barrier_fn barrier = nullptr; serfsim_allreduce_u64_fn allreduce = nullptr; void* comm_user = nullptr;
-  std::vector<IpcMapping> ipc_opened;
+  // the cross-shard exchange of a sharded run (world_size > 1), allocated together by serfsim_create; peer tables hold MAX_WORLD pointers
+  struct Exchange {
+    DevArray<u64> win_data[2];     // my receive windows [parity][world][win_cap]  (IPC-exported)
+    DevArray<u32> ctrl;            // my control block [parity][counts[8] | flags[8]] (IPC-exported)
+    DevArray<u32> send_count;      // [world] entries written into each peer's window this tick
+    DevArray<u64*> peer_data[2];   // device arrays of peer window pointers, per parity
+    DevArray<u32*> peer_ctrl; DevArray<u8*> peer_anomaly;   // … of peer control-block pointers, of every rank's injector flag array
+    DevArray<const uint4*> peer_snap_rec; DevArray<const u64*> peer_snap_node;   // push-pull rounds: … of every rank's snapshot pointers
+    DevArray<u64> grow;            // [trace_cap][8] global trace rows, summed on the device by the drain kernel (grown by ensure_trace)
+    u32 epoch = 0;                 // executed-tick counter (never rewinds): stamps and parity
+    u32 win_cap = 0, win_cap_base = 0;   // entries per peer segment; win_cap_base: sized for the membership entries alone (serfsim_create)
+    bool connected = false, loopback = false;   // loopback: serfsim_comm_loopback, a profiling aid: the handle exchanges with itself
+    serfsim_barrier_fn barrier = nullptr; serfsim_allreduce_u64_fn allreduce = nullptr; void* user = nullptr;   // both or neither
+    std::vector<IpcMapping> ipc;   // peers' buffers mapped by serfsim_comm_connect
+    std::vector<Event> mid_ev;     // after the tick kernel (breakdown of a timed run, SERFSIM_XTIMING=1)
+  };
+  std::optional<Exchange> xc;
   bool tick_timing = false;
   size_t l2_persist_max = 0, l2_window_max = 0;
   // asynchronous result read-back (serfsim_results_async): extraction into a ring of staging buffers on the launch stream,
@@ -269,7 +270,6 @@ struct serfsim {
   struct ReadBack { Stream copy_stream; Event extracted; ResBuf res[4]; u32 next = 0; };
   std::optional<ReadBack> rb;      // allocated together by the first serfsim_results_async
   std::vector<Event> tick_ev;      // 2 per tick when tick_timing
-  std::vector<Event> mid_ev;       // after the tick kernel (multi-GPU breakdown, SERFSIM_XTIMING=1)
 };
 
 namespace {
@@ -286,7 +286,7 @@ int ensure_trace(serfsim* h, u32 need) {
   CU(h->d_trace.grow((size_t)cap * ROW_FIELDS, h->stream));
   CU(h->d_kinds.grow(((size_t)cap + 1) * 4, h->stream));
   CU(h->d_view_kinds.grow(((size_t)cap + 1) * h->R * 4, h->stream));
-  if (h->cfg.world_size > 1) CU(h->d_grow.grow((size_t)cap * ROW_FIELDS, h->stream));
+  if (h->xc) CU(h->xc->grow.grow((size_t)cap * ROW_FIELDS, h->stream));
   h->trace_cap = cap;
   return 0;
 }
@@ -338,7 +338,7 @@ bool pp_tick(const serfsim* h, u32 t) {         // an anti-entropy round follows
 enum class TickRun { General, Passes, Check, Dual };
 TickRun tick_run(const serfsim* h, u32 t) {
   if (!h->sw.sv || h->R < 2 || h->R >= 32 || h->cfg.trace || h->sw.no_skip || h->byz_on) return TickRun::General;
-  if (h->cfg.world_size > 1) {
+  if (h->xc) {
     if (__builtin_popcount(h->ever_down) != 1) return TickRun::General;
     return h->sw.sv == 2 ? TickRun::Check : TickRun::Dual;
   }
@@ -371,16 +371,30 @@ int grow_events(std::vector<Event>& ev, size_t n) {
   return 0;
 }
 
+// The host collectives of a sharded run (hooks of serfsim_comm_set_hooks, installed both or neither); nothing to do when unsharded.
+const char* const kNoHooks = "world_size > 1: serfsim_comm_set_hooks was not called";
+int cluster_barrier(serfsim* h) {
+  if (!h->xc) return 0;
+  if (!h->xc->barrier) return fail(SERFSIM_E_COMM, kNoHooks);
+  h->xc->barrier(h->xc->user);
+  return 0;
+}
+int cluster_sum(serfsim* h, u64* v, u32 n) {     // v[0, n) summed over the ranks, in place
+  if (!h->xc) return 0;
+  if (!h->xc->allreduce) return fail(SERFSIM_E_COMM, kNoHooks);
+  h->xc->allreduce(h->xc->user, v, n);
+  return 0;
+}
+
 // The tracked user events' Lamport times as the cluster knows them: the origin's shard stamps an event, the other shards may not have it
 // yet, so each contributes the stamps of its own nodes' events and every rank gets the sum (a collective when sharded).  Stream idle.
 int ue_cluster_ltimes(serfsim* h, u32 lt[MAX_UEVENTS]) {
   CU(cudaMemcpy(lt, h->ue->ltime, h->ue->ltime.bytes(), cudaMemcpyDeviceToHost));
-  if (h->cfg.world_size > 1 && h->allreduce) {
-    u64 v[MAX_UEVENTS];
-    for (u32 e = 0; e < MAX_UEVENTS; ++e) v[e] = (((h->ue_injected >> e) & 1u) && h->ue_origin[e] - h->first < h->count) ? lt[e] : 0;
-    h->allreduce(h->comm_user, v, MAX_UEVENTS);
-    for (u32 e = 0; e < MAX_UEVENTS; ++e) lt[e] = (u32)v[e];
-  }
+  if (!h->xc) return 0;
+  u64 v[MAX_UEVENTS];
+  for (u32 e = 0; e < MAX_UEVENTS; ++e) v[e] = (((h->ue_injected >> e) & 1u) && h->ue_origin[e] - h->first < h->count) ? lt[e] : 0;
+  if (int rc = cluster_sum(h, v, MAX_UEVENTS)) return rc;
+  for (u32 e = 0; e < MAX_UEVENTS; ++e) lt[e] = (u32)v[e];
   return 0;
 }
 
@@ -426,15 +440,15 @@ TickParams tick_params(const serfsim* h, u32 t, OpRange ops) {
   p.sleep_on = (h->sw.no_skip || h->byz_on) ? 0u : 1u;          // injectors send every tick: the cluster never sleeps
   p.pp_every = (u32)std::max(0, h->cfg.push_pull_interval_ticks); p.reap_every = h->cfg.reap_interval_ticks;
   p.host_idle_until = h->d_pin_ctl + 2;
-  const bool sharded = h->cfg.world_size > 1;
-  const u32 xpar = h->xepoch & 1;
-  p.world = (u32)h->cfg.world_size; p.rank = (u32)h->cfg.rank; p.shard_size = h->shard_size; p.win_cap = h->win_cap;
-  p.win_data = h->d_peer_data[xpar]; p.send_count = h->d_send_count;
-  p.peer_ctrl = h->d_peer_ctrl; p.stamp = h->xepoch + 1; p.xpar = xpar; p.loopback = h->loopback ? 1u : 0u;
-  p.fuse_publish = (sharded && !h->byz_on && !h->sw.no_fuse) ? 1u : 0u;
+  p.world = (u32)h->cfg.world_size; p.rank = (u32)h->cfg.rank; p.shard_size = h->shard_size; p.stamp = 1;
+  if (const auto& x = h->xc) {                     // unsharded runs: no windows, parity 0, stamp 1
+    p.xpar = x->epoch & 1; p.stamp = x->epoch + 1; p.loopback = x->loopback ? 1u : 0u;
+    p.win_cap = x->win_cap; p.win_data = x->peer_data[p.xpar]; p.send_count = x->send_count; p.peer_ctrl = x->peer_ctrl;
+    p.fuse_publish = (!h->byz_on && !h->sw.no_fuse) ? 1u : 0u;
+  }
   p.shard_inv = (u32)(0x100000000ull / h->shard_size); p.xcap = p.world > 1 ? XW_TOTAL / (p.world - 1) : 0u;
   if (h->gate_on) {                                // convergence gate: the first kernel of the tick evaluates the row of tick t-1
-    const u64* grow = sharded ? h->d_grow : h->d_trace;            // global rows: the device sums them when sharded
+    const u64* grow = h->xc ? h->xc->grow : h->d_trace;            // global rows: the device sums them when sharded
     Gate& g = p.gate;
     g.ctl = h->d_runctl; g.host_ctl = h->d_pin_ctl; g.prev_row = t > h->gate_first ? grow + (size_t)(t - 1) * ROW_FIELDS : nullptr; g.tick = t;
     g.future_ops = (t > 0 && future_ops(h, t - 1)) ? 1u : 0u;
@@ -454,8 +468,8 @@ void launch_user_events(serfsim* h, const TickParams& p) {
   u.ltime = h->ue->ltime; u.node_state = h->d_node; u.busy = h->d_busy; u.row_ptr = h->d_rowptr; u.col = h->d_col;
   u.ev_node = h->d_ev_node; u.ev_op = h->d_ev_op; u.ev_slot = h->d_ev_slot;
   u.row = p.row; u.totals = h->ue->totals; u.overflow = h->d_overflow; u.sched = h->d_sched;
-  u.world = p.world; u.rank = p.rank; u.shard_size = h->shard_size; u.win_cap = h->win_cap;
-  u.win_data = p.win_data; u.send_count = h->d_send_count;
+  u.world = p.world; u.rank = p.rank; u.shard_size = h->shard_size; u.win_cap = p.win_cap;
+  u.win_data = p.win_data; u.send_count = p.send_count;
   u.gate = p.gate; u.gate.evaluate = 1u;
   launch_uevent(u, h->cfg.trace != 0, h->stream);
   h->last_launches++;
@@ -503,31 +517,37 @@ void launch_injectors(serfsim* h, const TickParams& p) {
   b.seed_lo = p.seed_lo; b.seed_hi = p.seed_hi; b.delta = h->byz_delta; b.ids = h->byz->ids; b.rec = h->d_rec; b.node_state = h->d_node;
   b.row_ptr = h->d_rowptr; b.col = h->d_col; b.inbox_wr = h->d_inbox[t & 1]; b.hot_wr = h->d_hot[t & 1]; b.kinds_cur = p.kinds_cur;
   b.anomaly = h->byz->anomaly; b.totals = h->byz->totals;
-  b.n_local = h->count; b.world = p.world; b.rank = p.rank; b.shard_size = h->shard_size; b.win_cap = h->win_cap;
-  b.win_data = p.win_data; b.send_count = h->d_send_count; b.overflow = h->d_overflow; b.gate = p.gate.ctl;
+  b.n_local = h->count; b.world = p.world; b.rank = p.rank; b.shard_size = h->shard_size; b.win_cap = p.win_cap;
+  b.win_data = p.win_data; b.send_count = p.send_count; b.overflow = h->d_overflow; b.gate = p.gate.ctl;
   launch_byz(b, h->stream);
   h->last_launches++;
 }
 
 // The exchange of a sharded tick.  No host round trip: publish (counts + flag into every peer's control block) and drain (waits for the
 // peers' flags of this exchange) are ordinary kernels on the same stream.
-void launch_exchange(serfsim* h, const TickParams& p) {
+int launch_exchange(serfsim* h, const TickParams& p) {
+  serfsim::Exchange& x = *h->xc;
   const u32 t = p.tick, xpar = p.xpar;
+  if (h->tick_timing) {
+    if (int rc = grow_events(x.mid_ev, (size_t)t + 1)) return rc;
+    CU(cudaEventRecord(x.mid_ev[t], h->stream));
+  }
   PublishParams pb{};
-  pb.world = p.world; pb.rank = p.rank; pb.stamp = p.stamp; pb.xpar = xpar; pb.send_count = h->d_send_count; pb.peer_ctrl = h->d_peer_ctrl;
+  pb.world = p.world; pb.rank = p.rank; pb.stamp = p.stamp; pb.xpar = xpar; pb.send_count = x.send_count; pb.peer_ctrl = x.peer_ctrl;
   pb.row = p.row; pb.gate = p.gate.ctl; pb.sched = h->d_sched; pb.loopback = p.loopback;
   if (!p.fuse_publish) { launch_publish(pb, h->stream); h->last_launches++; }
   DrainParams d{};
-  d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.world; d.rank = p.rank; d.win_cap = h->win_cap; d.stamp = p.stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
-  d.win_data = h->d_win_data[xpar]; d.ctrl = h->d_ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
-  d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = h->d_peer_anomaly;
+  d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.world; d.rank = p.rank; d.win_cap = x.win_cap; d.stamp = p.stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
+  d.win_data = x.win_data[xpar]; d.ctrl = x.ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
+  d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = x.peer_anomaly;
   d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->ue->inbox[t & 1].get() : nullptr; d.ue_ltime = h->ue ? h->ue->ltime.get() : nullptr;
-  d.my_row = p.row; d.grow = h->d_grow + (size_t)t * ROW_FIELDS; d.gate = p.gate.ctl;
-  d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(h->d_ctrl.get()) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
+  d.my_row = p.row; d.grow = x.grow + (size_t)t * ROW_FIELDS; d.gate = p.gate.ctl;
+  d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(x.ctrl.get()) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
   d.sched = h->d_sched; d.sched_rw = h->d_sched; d.host_idle_until = h->d_pin_ctl + 2; d.tick = t; d.sleep_on = p.sleep_on;
   launch_drain(d, h->stream);
   h->last_launches += 1;
-  h->xepoch++;
+  x.epoch++;
+  return 0;
 }
 
 // Anti-entropy round on a snapshot of the end-of-tick state (only this node's own records are written); p: as the membership tick left it.
@@ -540,13 +560,13 @@ int anti_entropy_round(serfsim* h, TickParams p) {
     p.ue_table = h->ue_table; p.ue_state = h->ue->state; p.ue_snap = h->ue->snap; p.ue_snap_peer = h->ue->peer_snap;
     p.ue_ltime = h->ue->ltime; p.ue_totals = h->ue->totals;
   }
-  if (h->cfg.world_size > 1) {
+  if (h->xc) {
     // partners may live on other GPUs: their snapshots are read through the peer mappings.  Rounds are rare (every
     // push_pull_interval ticks) and always the first tick of a convergence chunk, so two host barriers are affordable:
     // every rank has taken its snapshot before anyone reads, everyone has read before anyone moves on.
-    p.snap_rec_peer = h->d_peer_snap_rec; p.snap_node_peer = h->d_peer_snap_node;
+    p.snap_rec_peer = h->xc->peer_snap_rec; p.snap_node_peer = h->xc->peer_snap_node;
     CU(cudaStreamSynchronize(h->stream));
-    h->barrier(h->comm_user);
+    if (int rc = cluster_barrier(h)) return rc;
     if (h->ue_table.n) {
       // A partner in another shard may hold events this shard has never received, so their Lamport times are not in the
       // local table yet (a shard learns them from the first window entry of the event).  The replay needs them: every rank
@@ -555,17 +575,17 @@ int anti_entropy_round(serfsim* h, TickParams p) {
       if (int rc = ue_cluster_ltimes(h, lt)) return rc;
       CU(cudaMemcpy(h->ue->ltime, lt, h->ue->ltime.bytes(), cudaMemcpyHostToDevice));
     }
-    launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
+  }
+  launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
+  if (h->xc) {
     CU(cudaStreamSynchronize(h->stream));
-    h->barrier(h->comm_user);
+    if (int rc = cluster_barrier(h)) return rc;
     // the round changed this rank's row (changed / pending / hash) after the drain kernel summed the rows: redo the sum through
     // the host hook — the host is in the loop here anyway (two barriers), and rounds are rare
     u64 row[ROW_FIELDS];
     CU(cudaMemcpy(row, h->d_trace + (size_t)t * ROW_FIELDS, sizeof(row), cudaMemcpyDeviceToHost));
-    h->allreduce(h->comm_user, row, ROW_FIELDS);
-    CU(cudaMemcpy(h->d_grow + (size_t)t * ROW_FIELDS, row, sizeof(row), cudaMemcpyHostToDevice));
-  } else {
-    launch_pushpull(p, h->d_snap_rec, h->d_snap_node, h->cfg.trace != 0, h->stream);
+    if (int rc = cluster_sum(h, row, ROW_FIELDS)) return rc;
+    CU(cudaMemcpy(h->xc->grow + (size_t)t * ROW_FIELDS, row, sizeof(row), cudaMemcpyHostToDevice));
   }
   h->last_launches++;
   return 0;
@@ -574,7 +594,7 @@ int anti_entropy_round(serfsim* h, TickParams p) {
 // Launch n ticks on the stream (no synchronisation).
 int launch_ticks(serfsim* h, u32 n) {
   if (!h->has_topo) return fail(SERFSIM_E_INVAL, "serfsim_step: no topology set");
-  if (h->cfg.world_size > 1 && !h->connected) return fail(SERFSIM_E_COMM, "serfsim_step: world_size > 1 but serfsim_comm_connect was not called");
+  if (h->xc && !h->xc->connected) return fail(SERFSIM_E_COMM, "serfsim_step: world_size > 1 but serfsim_comm_connect was not called");
   int rc = upload_ops(h);
   if (rc) return rc;
   rc = ensure_trace(h, h->tick + n + 1);
@@ -608,13 +628,7 @@ int launch_ticks(serfsim* h, u32 n) {
     if (h->ue_table.n) launch_user_events(h, p);
     launch_membership(h, p);
     if (h->byz_n) launch_injectors(h, p);
-    if (h->cfg.world_size > 1) {
-      if (h->tick_timing) {
-        if ((rc = grow_events(h->mid_ev, (size_t)t + 1))) return rc;
-        CU(cudaEventRecord(h->mid_ev[t], h->stream));
-      }
-      launch_exchange(h, p);
-    }
+    if (h->xc && (rc = launch_exchange(h, p))) return rc;
     if (pp_tick(h, t) && (rc = anti_entropy_round(h, p))) return rc;
     if (h->tick_timing) CU(cudaEventRecord(h->tick_ev[2 * (size_t)t + 1], h->stream));
     h->launch_log.push_back((u32)(h->last_launches - launches_before));
@@ -635,7 +649,8 @@ int finish_timing(serfsim* h) {
 }
 
 int check_overflow(serfsim* h) {
-  if (h->ue_table.n) {
+  // without hooks a sharded handle never connected, so no tick ran and no event fired (run_until_converged with max_ticks = 0 gets here)
+  if (h->ue_table.n && (!h->xc || h->xc->allreduce)) {
     // Cluster runs need one Lamport time per ring slot: the packed event record derives a slot's ltime from the events in it.
     // (Two tracked events 512·k apart would alias — the quirk itself is kept in ue_handle and pinned by the handler tests.)
     u32 lt[MAX_UEVENTS];
@@ -661,8 +676,8 @@ int pull_rows(serfsim* h) {                     // bring rows [rows.size(), tick
   if (have >= h->tick) return 0;
   const u32 n = h->tick - have;
   h->rows.resize(h->tick);
-  // sharded runs: the drain kernel of every tick has already summed the ranks' rows on the device (d_grow), no host collective
-  const u64* src = h->cfg.world_size > 1 ? h->d_grow : h->d_trace;
+  // sharded runs: the drain kernel of every tick has already summed the ranks' rows on the device (Exchange::grow), no host collective
+  const u64* src = h->xc ? h->xc->grow : h->d_trace;
   CU(cudaMemcpy(h->rows.data() + have, src + (size_t)have * ROW_FIELDS, (size_t)n * sizeof(serfsim_tick_row_t), cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -723,8 +738,8 @@ int do_reset(serfsim* h, u64 seed) {
   CU(h->d_tile_due.fill(0xff, h->stream)); CU(h->d_node_due.fill(0xff, h->stream));      // no timer runs
   CU(h->d_carry.fill(0, h->stream));                     // tags restart with the ticks
   CU(h->d_sched.fill(0, h->stream));
-  CU(h->d_trace.fill(0, h->stream)); CU(h->d_kinds.fill(0, h->stream)); CU(h->d_view_kinds.fill(0, h->stream)); CU(h->d_grow.fill(0, h->stream));
-  CU(h->d_runctl.fill(0, h->stream)); CU(h->d_send_count.fill(0, h->stream));
+  CU(h->d_trace.fill(0, h->stream)); CU(h->d_kinds.fill(0, h->stream)); CU(h->d_view_kinds.fill(0, h->stream));
+  CU(h->d_runctl.fill(0, h->stream)); if (h->xc) { CU(h->xc->grow.fill(0, h->stream)); CU(h->xc->send_count.fill(0, h->stream)); }
   { int rc = ue_reset(h); if (rc) return rc; }
   if (h->byz) { CU(h->byz->anomaly.fill(0, h->stream)); CU(h->byz->totals.fill(0, h->stream)); }
   { int rc = refresh_watchers(h); if (rc) return rc; }
@@ -739,7 +754,34 @@ int ipc_open(serfsim* h, const cudaIpcMemHandle_t& handle, const char* what, T**
   const cudaError_t e = m.create(handle);
   if (e != cudaSuccess) return fail(SERFSIM_E_COMM, std::string("cudaIpcOpenMemHandle(") + what + "): " + cudaGetErrorString(e));
   *out = (T*)(void*)m;
-  h->ipc_opened.push_back(std::move(m));
+  h->xc->ipc.push_back(std::move(m));
+  return 0;
+}
+
+// Every rank's exchange buffers as this rank addresses them, by rank (null where a rank has none), and their install into the device tables
+// the kernels read them from (the snapshot tables exist only with push-pull rounds on).
+struct PeerTables {
+  u64* data[2][MAX_WORLD] = {}; u32* ctrl[MAX_WORLD] = {}; u8* anomaly[MAX_WORLD] = {};
+  const uint4* snap_rec[MAX_WORLD] = {}; const u64* snap_node[MAX_WORLD] = {}; const uint4* ue_snap[MAX_WORLD] = {};
+};
+int install_peers(serfsim* h, const PeerTables& t) {
+  serfsim::Exchange& x = *h->xc;
+  auto put = [](auto& table, const auto* ptrs) { return cudaMemcpy(table, ptrs, table.bytes(), cudaMemcpyHostToDevice); };
+  for (int par = 0; par < 2; ++par) CU(put(x.peer_data[par], t.data[par]));
+  CU(put(x.peer_ctrl, t.ctrl)); CU(put(x.peer_anomaly, t.anomaly));
+  if (x.peer_snap_rec) { CU(put(x.peer_snap_rec, t.snap_rec)); CU(put(x.peer_snap_node, t.snap_node)); }
+  if (h->ue && h->ue->peer_snap) CU(put(h->ue->peer_snap, t.ue_snap));
+  return 0;
+}
+
+// Receive windows for n_events tracked user events, zeroed (they read as zeros wherever nothing was written).  Per peer: win_cap_base membership
+// entries (sized once, by serfsim_create: the grids may change later) plus one per event bit bound for another shard, up to fanout · n_events per node and tick.
+int size_windows(serfsim* h, serfsim::Exchange& x, u32 n_events) {
+  const u32 want = (u32)std::min((double)x.win_cap_base + (double)h->shard_size * h->cfg.fanout * n_events * h->sw.win_factor / h->cfg.world_size, 4.0e9);
+  if (want == x.win_cap) return 0;
+  if (x.connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs call it before serfsim_comm_export / serfsim_comm_connect (it resizes the receive windows)");
+  for (int par = 0; par < 2; ++par) { CU(x.win_data[par].alloc((size_t)h->cfg.world_size * want)); CU(x.win_data[par].fill(0, h->stream)); }
+  x.win_cap = want;
   return 0;
 }
 
@@ -876,26 +918,21 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   }
   if (cfg->world_size > 1) {
     // receive windows: one segment per peer; expected entries per tick and pair ≈ shard · fanout · R · kinds / world
-    if (cfg->world_size > 8) return fail(SERFSIM_E_INVAL, "world_size > 8");
+    if (cfg->world_size > MAX_WORLD) return fail(SERFSIM_E_INVAL, "world_size > 8");
+    serfsim::Exchange x;
     // … plus what a warp of the tick kernel (TILE threads) can leave unfilled in a peer's window: its reservation ahead and a partial block
     const double pad = (double)std::max(h->grid, h->grid_sv) * (TILE / 32) * (XW_RESERVE_MAX + XW_FLUSH);   // (the single-view kernel of a multi-slot run has the larger grid)
-    double cap = (double)h->shard_size * cfg->fanout * h->R * 3.0 * h->sw.win_factor / cfg->world_size + 4096.0 + pad;
-    h->win_cap = (u32)std::min(cap, 4.0e9);
-    h->win_cap_base = h->win_cap;
-    for (int par = 0; par < 2; ++par) {
-      CU(h->d_win_data[par].alloc((size_t)cfg->world_size * h->win_cap));
-      CU(h->d_win_data[par].fill(0, h->stream));      // windows read as zeros wherever nothing was written
-      CU(h->d_peer_data[par].alloc(8));
-    }
-    CU(h->d_ctrl.alloc(CTRL_BYTES / sizeof(u32))); CU(h->d_ctrl.fill(0, h->stream));
-    CU(h->d_send_count.alloc(8));
-    CU(h->d_peer_ctrl.alloc(8));
+    x.win_cap_base = (u32)std::min((double)h->shard_size * cfg->fanout * h->R * 3.0 * h->sw.win_factor / cfg->world_size + 4096.0 + pad, 4.0e9);
+    if (int rc = size_windows(h.get(), x, 0)) return rc;
+    for (int par = 0; par < 2; ++par) CU(x.peer_data[par].alloc(MAX_WORLD));
+    CU(x.ctrl.alloc(CTRL_BYTES / sizeof(u32))); CU(x.ctrl.fill(0, h->stream));
+    CU(x.send_count.alloc(MAX_WORLD)); CU(x.peer_ctrl.alloc(MAX_WORLD)); CU(x.peer_anomaly.alloc(MAX_WORLD));
+    if (cfg->push_pull_interval_ticks > 0) { CU(x.peer_snap_rec.alloc(MAX_WORLD)); CU(x.peer_snap_node.alloc(MAX_WORLD)); }
+    h->xc = std::move(x);
     serfsim::Injectors b; CU(b.anomaly.alloc(h->stride)); CU(b.totals.alloc(4)); h->byz = std::move(b);   // peers' drain kernels raise the flags
-    CU(h->d_peer_anomaly.alloc(8));
   }
   if (cfg->push_pull_interval_ticks > 0) {         // push-pull rounds' snapshots (sharded runs export them, so all are allocated here)
     CU(h->d_snap_rec.alloc(h->d_rec.size())); CU(h->d_snap_node.alloc(h->d_node.size()));
-    if (cfg->world_size > 1) { CU(h->d_peer_snap_rec.alloc(8)); CU(h->d_peer_snap_node.alloc(8)); }
   }
   if (int rc = ensure_trace(h.get(), 1024)) return rc;
   if (int rc = do_reset(h.get(), cfg->seed)) return rc;
@@ -906,11 +943,12 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
 void serfsim_destroy(serfsim_t* h) {
   if (!h) return;
   cudaStreamSynchronize(h->stream);
-  if (h->sw.xtiming && !h->mid_ev.empty()) {
-    double a = 0, b = 0; size_t n = std::min(h->mid_ev.size(), h->tick_ev.size() / 2);
+  if (h->sw.xtiming && h->xc && !h->xc->mid_ev.empty()) {
+    const std::vector<Event>& mid = h->xc->mid_ev;
+    double a = 0, b = 0; size_t n = std::min(mid.size(), h->tick_ev.size() / 2);
     for (size_t t = 0; t < n; ++t) {
       float x = 0, y = 0;
-      if (cudaEventElapsedTime(&x, h->tick_ev[2 * t], h->mid_ev[t]) == cudaSuccess && cudaEventElapsedTime(&y, h->mid_ev[t], h->tick_ev[2 * t + 1]) == cudaSuccess) {
+      if (cudaEventElapsedTime(&x, h->tick_ev[2 * t], mid[t]) == cudaSuccess && cudaEventElapsedTime(&y, mid[t], h->tick_ev[2 * t + 1]) == cudaSuccess) {
         a += x; b += y;
         if (t >= 12 && t <= 15) fprintf(stderr, "rank %d tick %zu: tick kernel %.1f us, publish+drain %.1f us\n", h->cfg.rank, t, x * 1e3, y * 1e3);
       }
@@ -1041,7 +1079,7 @@ int serfsim_run_until_converged(serfsim_t* h, uint32_t max_ticks, uint32_t* tick
   };
   auto stop_at = [&](u32 t) {                         // tick t is the first quiescent one: later launches did not execute
     const u32 skipped = h->tick - (t + 1);
-    if (h->cfg.world_size > 1) h->xepoch -= skipped;   // skipped ticks exchanged nothing
+    if (h->xc) h->xc->epoch -= skipped;                // skipped ticks exchanged nothing
     h->tick = t + 1;
     if (h->rows.size() > h->tick) h->rows.resize(h->tick);
     u64 executed = 0;                                  // kernels of the ticks that did run (launch_log starts at launch_log_first)
@@ -1077,7 +1115,7 @@ int serfsim_run_until_converged(serfsim_t* h, uint32_t max_ticks, uint32_t* tick
       const u32 n_skip = std::min(stop > h->tick ? stop - h->tick : 0u, max_ticks - (h->tick - start));
       if (n_skip) {
         if ((rc = ensure_trace(h, h->tick + n_skip + 1))) return rc;
-        launch_fill_idle_rows(h->d_trace + (size_t)h->tick * 8, h->cfg.world_size > 1 ? h->d_grow + (size_t)h->tick * 8 : nullptr, n_skip, h->d_sched, h->cfg.trace != 0, h->stream);
+        launch_fill_idle_rows(h->d_trace + (size_t)h->tick * 8, h->xc ? h->xc->grow + (size_t)h->tick * 8 : nullptr, n_skip, h->d_sched, h->cfg.trace != 0, h->stream);
         h->last_launches++;
         SFS_COUNT(17, n_skip);                           // ticks the host jumped over
         for (u32 k = 0; k < n_skip; ++k) {
@@ -1185,11 +1223,7 @@ int serfsim_state_hash(serfsim_t* h, uint64_t* out) {
   CU(cudaMemcpyAsync(parts, h->d_scratch, 4 * 8, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   *out = parts[0] + parts[3];                    // records + node words, plus the event records when user events are on
-  if (h->cfg.world_size > 1) {
-    if (!h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
-    h->allreduce(h->comm_user, out, 1);
-  }
-  return 0;
+  return cluster_sum(h, out, 1);
 }
 
 int serfsim_stats(serfsim_t* h, serfsim_stats_t* o) {
@@ -1217,7 +1251,7 @@ int serfsim_set_byzantine(serfsim_t* h, uint32_t n, const uint32_t* ids, uint32_
   if (!h) return fail(SERFSIM_E_INVAL, "null handle");
   if (n && !ids) return fail(SERFSIM_E_INVAL, "null ids");
   if (h->tick != 0 || !h->ops.empty()) return fail(SERFSIM_E_INVAL, "serfsim_set_byzantine: call before any operation is scheduled (or after serfsim_reset)");
-  if (n && h->cfg.world_size > 1 && h->shard_size >= BYZ_FLAG) return fail(SERFSIM_E_INVAL, "byzantine injectors: shards must hold fewer than 2^25 nodes");
+  if (n && h->xc && h->shard_size >= BYZ_FLAG) return fail(SERFSIM_E_INVAL, "byzantine injectors: shards must hold fewer than 2^25 nodes");
   std::vector<u32> v(ids, ids + n);
   std::sort(v.begin(), v.end());
   for (u32 i = 0; i < n; ++i) if (v[i] >= h->N || (i && v[i] == v[i - 1])) return fail(SERFSIM_E_INVAL, "byzantine ids must be distinct node ids");
@@ -1239,10 +1273,7 @@ int serfsim_anomaly_flags(serfsim_t* h, uint8_t* out) {
   if (!h || !out) return fail(SERFSIM_E_INVAL, "null argument");
   if (!h->byz_on) return fail(SERFSIM_E_INVAL, "no byzantine injectors set (serfsim_set_byzantine)");
   CU(cudaStreamSynchronize(h->stream));
-  if (h->cfg.world_size > 1) {                     // peers' drain kernels raise flags in this array: wait until every rank has drained
-    if (!h->barrier) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
-    h->barrier(h->comm_user);
-  }
+  if (int rc = cluster_barrier(h)) return rc;     // peers' drain kernels raise flags in this array: wait until every rank has drained
   CU(cudaMemcpy(out, h->byz->anomaly, h->count, cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -1252,16 +1283,13 @@ int serfsim_byzantine_stats(serfsim_t* h, serfsim_byz_stats_t* o) {
   if (!h->byz_on) return fail(SERFSIM_E_INVAL, "no byzantine injectors set (serfsim_set_byzantine)");
   u64 t[4] = {0, 0, 0, 0};
   CU(cudaStreamSynchronize(h->stream));
-  if (h->cfg.world_size > 1) {
-    if (!h->barrier || !h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
-    h->barrier(h->comm_user);                      // see serfsim_anomaly_flags
-  }
+  if (int rc = cluster_barrier(h)) return rc;     // see serfsim_anomaly_flags
   CU(cudaMemcpy(t, h->byz->totals, h->byz->totals.bytes(), cudaMemcpyDeviceToHost));
   std::vector<u8> flags(h->count);
   CU(cudaMemcpy(flags.data(), h->byz->anomaly, h->count, cudaMemcpyDeviceToHost));
   u64 v[3] = {t[0], t[1], 0};
   for (u8 f : flags) v[2] += f ? 1 : 0;
-  if (h->cfg.world_size > 1) h->allreduce(h->comm_user, v, 3);
+  if (int rc = cluster_sum(h, v, 3)) return rc;
   o->messages = v[0]; o->edge_updates = v[1]; o->flagged = v[2];
   return 0;
 }
@@ -1272,24 +1300,14 @@ int serfsim_set_user_events(serfsim_t* h, uint32_t n_events, const uint32_t* con
   if (n_events > MAX_UEVENTS) return fail(SERFSIM_E_INVAL, "at most SERFSIM_MAX_USER_EVENTS tracked user events");
   if (n_events && !content_ids) return fail(SERFSIM_E_INVAL, "null content ids");
   if (h->tick != 0 || !h->ops.empty()) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: call before any operation is scheduled (or after serfsim_reset)");
-  if (h->cfg.world_size > 1) {
-    // every event bit bound for another shard is one window entry: up to fanout · n_events per node and tick on top of the
-    // membership entries the windows were sized for.  The windows are exported by serfsim_comm_export, so this must come first.
-    const double cap = (double)h->win_cap_base + (double)h->shard_size * h->cfg.fanout * n_events * h->sw.win_factor / h->cfg.world_size;
-    const u32 want = (u32)std::min(cap, 4.0e9);
-    if (want != h->win_cap) {
-      if (h->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs call it before serfsim_comm_export / serfsim_comm_connect (it resizes the receive windows)");
-      for (int par = 0; par < 2; ++par) { CU(h->d_win_data[par].alloc((size_t)h->cfg.world_size * want)); CU(h->d_win_data[par].fill(0, h->stream)); }
-      h->win_cap = want;
-    }
-  }
+  if (h->xc) { if (int rc = size_windows(h, *h->xc, n_events)) return rc; }      // before serfsim_comm_export, which exports the windows
   if (n_events && !h->ue) {
     const bool pp = h->cfg.push_pull_interval_ticks > 0;
-    if (pp && h->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs with push-pull rounds call it before serfsim_comm_export (the event snapshot is exported)");
+    if (pp && h->xc && h->xc->connected) return fail(SERFSIM_E_INVAL, "serfsim_set_user_events: in sharded runs with push-pull rounds call it before serfsim_comm_export (the event snapshot is exported)");
     serfsim::UserEvents u;
     CU(u.state.alloc(h->stride)); CU(u.inbox[0].alloc(h->stride)); CU(u.inbox[1].alloc(h->stride));
     CU(u.ltime.alloc(MAX_UEVENTS)); CU(u.totals.alloc(8));
-    if (pp) { CU(u.snap.alloc(h->stride)); CU(u.peer_snap.alloc(8)); }
+    if (pp) { CU(u.snap.alloc(h->stride)); CU(u.peer_snap.alloc(MAX_WORLD)); }
     h->ue = std::move(u);
   }
   h->ue_table = UeTable{};
@@ -1373,7 +1391,6 @@ int serfsim_user_event_seen(serfsim_t* h, uint32_t event, uint8_t* out) {
 int serfsim_user_event_ltime(serfsim_t* h, uint32_t event, uint64_t* ltime) {
   if (!h || !ltime) return fail(SERFSIM_E_INVAL, "null argument");
   if (event >= h->ue_table.n) return fail(SERFSIM_E_INVAL, "user event index out of range");
-  if (h->cfg.world_size > 1 && !h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
   u32 lt[MAX_UEVENTS];
   CU(cudaStreamSynchronize(h->stream));
   if (int rc = ue_cluster_ltimes(h, lt)) return rc;
@@ -1400,10 +1417,7 @@ int serfsim_user_event_stats(serfsim_t* h, serfsim_uevent_stats_t* o) {
   CU(cudaMemcpyAsync(tot, h->ue->totals, h->ue->totals.bytes(), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
   u64 v[6] = {tot[0], tot[1], tot[2], tot[3], tot[4], sum[0]};
-  if (h->cfg.world_size > 1) {                      // counters are sums over shards; event_time (a maximum) stays shard-local
-    if (!h->allreduce) return fail(SERFSIM_E_COMM, "world_size > 1: serfsim_comm_set_hooks was not called");
-    h->allreduce(h->comm_user, v, 6);
-  }
+  if (int rc = cluster_sum(h, v, 6)) return rc;   // counters are sums over shards; event_time (a maximum) stays shard-local
   o->messages = v[0]; o->edge_updates = v[1]; o->delivered = v[2]; o->duplicates = v[3]; o->too_old = v[4];
   o->event_queue = v[5]; o->event_time = sum[1];
   return 0;
@@ -1454,13 +1468,13 @@ size_t serfsim_comm_blob_size(void) { return sizeof(comm_blob); }
 
 int serfsim_comm_export(serfsim_t* h, void* blob) {
   if (!h || !blob) return fail(SERFSIM_E_INVAL, "null argument");
-  if (h->cfg.world_size < 2) return fail(SERFSIM_E_INVAL, "world_size == 1: nothing to export");
+  if (!h->xc) return fail(SERFSIM_E_INVAL, "world_size == 1: nothing to export");
   comm_blob b{};
-  for (int par = 0; par < 2; ++par) CU(cudaIpcGetMemHandle(&b.data[par], h->d_win_data[par]));
-  CU(cudaIpcGetMemHandle(&b.ctrl, h->d_ctrl));
+  for (int par = 0; par < 2; ++par) CU(cudaIpcGetMemHandle(&b.data[par], h->xc->win_data[par]));
+  CU(cudaIpcGetMemHandle(&b.ctrl, h->xc->ctrl));
   CU(cudaIpcGetMemHandle(&b.anomaly, h->byz->anomaly));
   if (h->ue && h->ue->snap) { CU(cudaIpcGetMemHandle(&b.ue_snap, h->ue->snap)); b.has_ue_snap = 1; }
-  b.win_cap = h->win_cap; b.rank = (u32)h->cfg.rank;
+  b.win_cap = h->xc->win_cap; b.rank = (u32)h->cfg.rank;
 #ifndef SERFSIM_EMU
   { int dev = 0; cudaDeviceProp pr{}; CU(cudaGetDevice(&dev)); CU(cudaGetDeviceProperties(&pr, dev)); memcpy(b.dev_uuid, pr.uuid.bytes, 16); }
 #endif
@@ -1474,73 +1488,59 @@ int serfsim_comm_export(serfsim_t* h, void* blob) {
 
 int serfsim_comm_connect(serfsim_t* h, const void* blobs) {
   if (!h || !blobs) return fail(SERFSIM_E_INVAL, "null argument");
-  const int W = h->cfg.world_size;
-  if (W < 2) return fail(SERFSIM_E_INVAL, "world_size == 1");
-  if (!h->barrier || !h->allreduce) return fail(SERFSIM_E_COMM, "serfsim_comm_set_hooks must be called first");
+  if (!h->xc) return fail(SERFSIM_E_INVAL, "world_size == 1");
+  serfsim::Exchange& x = *h->xc;
+  if (!x.barrier || !x.allreduce) return fail(SERFSIM_E_COMM, "serfsim_comm_set_hooks must be called first");
   const comm_blob* bs = (const comm_blob*)blobs;
-  std::vector<u32*> pc(8, nullptr);
-  std::vector<std::vector<u64*>> pd(2, std::vector<u64*>(8, nullptr));
-  std::vector<const uint4*> psr(8, nullptr);
-  std::vector<const u64*> psn(8, nullptr);
-  std::vector<u8*> pan(8, nullptr);
-  std::vector<const uint4*> pus(8, nullptr);
+  PeerTables t;
   const uint4* ue_snap = h->ue ? h->ue->snap.get() : nullptr;
-  for (int r = 0; r < W; ++r) {
-    if (bs[r].rank != (u32)r || bs[r].win_cap != h->win_cap) return fail(SERFSIM_E_COMM, "blob order / window size mismatch");
+  for (int r = 0; r < h->cfg.world_size; ++r) {
+    if (bs[r].rank != (u32)r || bs[r].win_cap != x.win_cap) return fail(SERFSIM_E_COMM, "blob order / window size mismatch");
 #ifndef SERFSIM_EMU
     // one rank per GPU: the drain kernel spins on its peers' flags, and a peer that shares this GPU may never get an SM to raise them
-    for (int r2 = 0; r2 < r; ++r2) if (!h->loopback && memcmp(bs[r].dev_uuid, bs[r2].dev_uuid, 16) == 0) return fail(SERFSIM_E_COMM, "two ranks share one GPU (one process per GPU is required)");
+    for (int r2 = 0; r2 < r; ++r2) if (!x.loopback && memcmp(bs[r].dev_uuid, bs[r2].dev_uuid, 16) == 0) return fail(SERFSIM_E_COMM, "two ranks share one GPU (one process per GPU is required)");
 #endif
     if ((bs[r].has_snap != 0) != (h->d_snap_rec != nullptr)) return fail(SERFSIM_E_COMM, "push_pull_interval_ticks differs between ranks");
-    if (r == h->cfg.rank) { pd[0][r] = h->d_win_data[0]; pd[1][r] = h->d_win_data[1]; pc[r] = h->d_ctrl; psr[r] = h->d_snap_rec; psn[r] = h->d_snap_node; pan[r] = h->byz->anomaly; pus[r] = ue_snap; continue; }
+    if (r == h->cfg.rank) {
+      t.data[0][r] = x.win_data[0]; t.data[1][r] = x.win_data[1]; t.ctrl[r] = x.ctrl; t.anomaly[r] = h->byz->anomaly;
+      t.snap_rec[r] = h->d_snap_rec; t.snap_node[r] = h->d_snap_node; t.ue_snap[r] = ue_snap; continue;
+    }
     if ((bs[r].has_ue_snap != 0) != (ue_snap != nullptr)) return fail(SERFSIM_E_COMM, "user events / push-pull configuration differs between ranks");
-    int rc = bs[r].has_ue_snap ? ipc_open(h, bs[r].ue_snap, "event snapshot", &pus[r]) : 0;
-    if (!rc) rc = ipc_open(h, bs[r].anomaly, "flags", &pan[r]);
-    if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_rec, "snapshot", &psr[r]);
-    if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_node, "snapshot", &psn[r]);
-    for (int par = 0; par < 2 && !rc; ++par) rc = ipc_open(h, bs[r].data[par], "window", &pd[par][r]);
-    if (!rc) rc = ipc_open(h, bs[r].ctrl, "ctrl", &pc[r]);
+    int rc = bs[r].has_ue_snap ? ipc_open(h, bs[r].ue_snap, "event snapshot", &t.ue_snap[r]) : 0;
+    if (!rc) rc = ipc_open(h, bs[r].anomaly, "flags", &t.anomaly[r]);
+    if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_rec, "snapshot", &t.snap_rec[r]);
+    if (!rc && bs[r].has_snap) rc = ipc_open(h, bs[r].snap_node, "snapshot", &t.snap_node[r]);
+    for (int par = 0; par < 2 && !rc; ++par) rc = ipc_open(h, bs[r].data[par], "window", &t.data[par][r]);
+    if (!rc) rc = ipc_open(h, bs[r].ctrl, "ctrl", &t.ctrl[r]);
     if (rc) return rc;
   }
-  for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), h->d_peer_data[par].bytes(), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), h->d_peer_ctrl.bytes(), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_anomaly, pan.data(), h->d_peer_anomaly.bytes(), cudaMemcpyHostToDevice));
-  if (ue_snap) CU(cudaMemcpy(h->ue->peer_snap, pus.data(), h->ue->peer_snap.bytes(), cudaMemcpyHostToDevice));
-  if (h->d_snap_rec) {
-    CU(cudaMemcpy(h->d_peer_snap_rec, psr.data(), h->d_peer_snap_rec.bytes(), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(h->d_peer_snap_node, psn.data(), h->d_peer_snap_node.bytes(), cudaMemcpyHostToDevice));
-  }
-  h->barrier(h->comm_user);          // every rank has mapped every window before the first tick writes into one
-  h->connected = true;
+  if (int rc = install_peers(h, t)) return rc;
+  x.barrier(x.user);                 // every rank has mapped every window before the first tick writes into one
+  x.connected = true;
   return 0;
 }
 
 int serfsim_comm_loopback(serfsim_t* h) {
   if (!h) return fail(SERFSIM_E_INVAL, "null handle");
-  const int W = h->cfg.world_size;
-  if (W < 2) return fail(SERFSIM_E_INVAL, "world_size == 1");
+  if (!h->xc) return fail(SERFSIM_E_INVAL, "world_size == 1");
   if (h->cfg.rank != 0) return fail(SERFSIM_E_INVAL, "loopback: create the handle as rank 0");
   if (h->cfg.push_pull_interval_ticks > 0 || h->byz_on || h->ue_table.n) return fail(SERFSIM_E_INVAL, "loopback profiles the membership path only");
+  serfsim::Exchange& x = *h->xc;
   // entries for shard s are written at win_data[s][rank·win_cap + g]: with rank 0 the window of "peer" s is my own segment s
-  std::vector<u32*> pc(8, nullptr);
-  std::vector<std::vector<u64*>> pd(2, std::vector<u64*>(8, nullptr));
-  std::vector<u8*> pan(8, nullptr);
-  for (int r = 0; r < W; ++r) {
-    pc[r] = h->d_ctrl; pan[r] = h->byz->anomaly;
-    for (int par = 0; par < 2; ++par) pd[par][r] = h->d_win_data[par] + (size_t)r * h->win_cap;
+  PeerTables t;
+  for (int r = 0; r < h->cfg.world_size; ++r) {
+    t.ctrl[r] = x.ctrl; t.anomaly[r] = h->byz->anomaly;
+    for (int par = 0; par < 2; ++par) t.data[par][r] = x.win_data[par] + (size_t)r * x.win_cap;
   }
-  for (int par = 0; par < 2; ++par) CU(cudaMemcpy(h->d_peer_data[par], pd[par].data(), h->d_peer_data[par].bytes(), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_ctrl, pc.data(), h->d_peer_ctrl.bytes(), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->d_peer_anomaly, pan.data(), h->d_peer_anomaly.bytes(), cudaMemcpyHostToDevice));
-  h->barrier = [](void*) {};
-  h->allreduce = [](void*, uint64_t*, uint32_t) {};
-  h->connected = true; h->loopback = true;
+  if (int rc = install_peers(h, t)) return rc;
+  x.barrier = [](void*) {}; x.allreduce = [](void*, uint64_t*, uint32_t) {};
+  x.connected = true; x.loopback = true;
   return 0;
 }
 
 int serfsim_comm_set_hooks(serfsim_t* h, serfsim_barrier_fn barrier, serfsim_allreduce_u64_fn allreduce, void* user) {
   if (!h || !barrier || !allreduce) return fail(SERFSIM_E_INVAL, "null argument");
-  h->barrier = barrier; h->allreduce = allreduce; h->comm_user = user;
+  if (h->xc) { h->xc->barrier = barrier; h->xc->allreduce = allreduce; h->xc->user = user; }     // unsharded runs have no collectives
   return 0;
 }
 

@@ -5,6 +5,7 @@ SERFSIM_E_NOMEM and leaves a handle that, once the call is repeated, computes wh
 The shim counts the resources alive (emu_live_allocs) and makes the k-th next allocation fail (emu_fail_alloc_at).  The
 failure sweeps arm k = 1, 2, ... until the call makes fewer than k allocations, so every allocation of the call fails once."""
 import ctypes as C
+import gc
 import threading
 
 import numpy as np
@@ -39,6 +40,13 @@ def storm():
 
 def run(g, sc):
     g.run_until_converged(sc.max_ticks)
+
+
+def baseline(L):
+    """The resources alive before a measurement.  Handles that earlier tests of this process left in reference cycles are freed
+    first: the cycle collector could otherwise free them in the middle of the measurement."""
+    gc.collect()
+    return L.emu_live_allocs()
 
 
 # ---- part 1: every configuration releases what it allocated --------------------------------------------------------
@@ -134,7 +142,7 @@ CASES = {
 
 @pytest.mark.parametrize("case", sorted(CASES))
 def test_closed_handles_release_everything(L, case):
-    base = L.emu_live_allocs()
+    base = baseline(L)
     CASES[case]()
     assert L.emu_live_allocs() == base
 
@@ -151,7 +159,7 @@ def sweep(L, make, call, rest):
     """make() -> a handle ready for call(g) -> (rc, value); rest(g, value) -> the outputs the handle then computes.  For every
     allocation of call: it fails with SERFSIM_E_NOMEM, the repeated call succeeds, the outputs equal those of a handle whose
     call never failed, and every handle releases everything.  Returns the number of allocations the call makes."""
-    base = L.emu_live_allocs()
+    base = baseline(L)
     g = make()
     rc, value = call(g)
     assert rc == 0, rc
@@ -213,7 +221,7 @@ def test_create_fails_cleanly_at_every_allocation(L, cfg):
     """serfsim_create, including the push-pull snapshots (allocated by create so that a round never allocates mid-tick)."""
     cfg = dict(cfg)
     slots = cfg.pop("slots", 1)
-    base = L.emu_live_allocs()
+    base = baseline(L)
     k = 1
     while True:
         L.emu_fail_alloc_at(k)

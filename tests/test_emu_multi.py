@@ -123,6 +123,48 @@ def test_sharded_byzantine_with_push_pull():
     P.run_against_oracle(emu_sim, scenarios.byzantine_injectors(2400, 12, 3, 0.05, seed=5), world=3, push_pull_interval_ticks=6)
 
 
+def test_sharded_handle_without_hooks_or_connection():
+    """A world-2 handle whose host never installed the collective hooks: every call that needs a barrier or an all-reduce fails
+    with SERFSIM_E_COMM instead of returning a shard-local answer, and a step fails because the handle is not connected.  A run of
+    zero ticks launches nothing and reports "not converged at tick 0", user events or not.  Once the handle is connected, user
+    events that need bigger receive windows are refused (the windows were exported already)."""
+    from serf_b200.sim import SerfsimError
+    E_INVAL, E_COMM = -1, -6
+
+    def error(f, *args):
+        with pytest.raises(SerfsimError) as ei:
+            f(*args)
+        return ei.value
+
+    def code(f, *args):
+        return error(f, *args).code
+
+    sc = scenarios.random_graph_leave(600, 8, 3, seed=2, slots=1)
+
+    def handle():
+        g = emu_sim(sc.n, sc.slots, rank=0, world_size=2, **sc.cfg)
+        g.set_topology(sc.row_ptr, sc.col)
+        return g
+
+    g = handle()
+    g.set_user_events([1, 2])
+    g.set_byzantine([1, 400])
+    assert code(g.state_hash) == E_COMM
+    assert code(g.user_event_stats) == E_COMM
+    assert code(g.user_event_ltime, 0) == E_COMM
+    assert code(g.anomaly_flags) == E_COMM
+    assert code(g.byzantine_stats) == E_COMM
+    assert code(g.step, 1) == E_COMM
+    assert g.run_until_converged(0) == (0, False)
+    g.close()
+
+    g = handle()
+    g.connect_loopback()
+    e = error(g.set_user_events, [1, 2, 3])
+    assert e.code == E_INVAL and "resizes the receive windows" in str(e), str(e)
+    g.close()
+
+
 def test_loopback_profiling_aid_runs():
     """serfsim_comm_loopback: a world-4 handle exchanging with itself (tools/loopback_profile.py).  Its results are meaningless by
     construction; what is checked is that the sharded kernels run to quiescence through the windows without an error."""
