@@ -38,9 +38,10 @@ __global__ void __launch_bounds__(128) byz_kernel(const __grid_constant__ ByzPar
         for (u32 k = 0; k < nt; ++k) {
           const u32 dl = tg[k] - p.first;
           n_msgs += 2; n_edges += 1;
-          if (p.world > 1 && dl >= p.n_local) {                // the peer lives in another shard: triple into its window
-            const u32 shard = tg[k] / p.shard_size, dloc = (tg[k] - shard * p.shard_size) | BYZ_FLAG;
-            win_append<3>(p, shard, {win_entry(serf_val1, s, e.serf_kind, dloc), win_entry(e.ml_key + 1u, s, KIND_ML, dloc),
+          if (p.snd.world > 1 && dl >= p.n_local) {                // the peer lives in another shard: triple into its window
+            const ShardIdx t = shard_of(tg[k], p.snd.shard_size, p.snd.shard_inv);
+            const u32 dloc = t.local | BYZ_FLAG;
+            win_append<3>(p.snd, p.overflow, t.shard, {win_entry(serf_val1, s, e.serf_kind, dloc), win_entry(e.ml_key + 1u, s, KIND_ML, dloc),
                                      win_entry(u + 1u, BYZ_ANNOT_SLOT, KIND_EXTRA, dloc)});
             wrote_remote = true;
             continue;                                          // kinds / tile flags / verdict are the receiving shard's business

@@ -39,7 +39,6 @@ thread_local std::string g_err;
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
 struct HostOp { u32 tick, op, node, slot; u64 seq; };
-constexpr int MAX_WORLD = 8;     // ranks of a sharded run
 
 // memberlist retransmit limit: retransmit_mult * ceil(log10(n + 1))  [external crate, restated].  In 64 bits: serfsim_create
 // rejects a product outside 1..255 (the budgets are u8) instead of letting it wrap in u32.
@@ -440,13 +439,14 @@ TickParams tick_params(const serfsim* h, u32 t, OpRange ops) {
   p.sleep_on = (h->sw.no_skip || h->byz_on) ? 0u : 1u;          // injectors send every tick: the cluster never sleeps
   p.pp_every = (u32)std::max(0, h->cfg.push_pull_interval_ticks); p.reap_every = h->cfg.reap_interval_ticks;
   p.host_idle_until = h->d_pin_ctl + 2;
-  p.world = (u32)h->cfg.world_size; p.rank = (u32)h->cfg.rank; p.shard_size = h->shard_size; p.stamp = 1;
+  Sender& snd = p.snd;
+  snd.world = (u32)h->cfg.world_size; snd.rank = (u32)h->cfg.rank; snd.shard_size = h->shard_size; snd.shard_inv = shard_recip(h->shard_size); p.stamp = 1;
   if (const auto& x = h->xc) {                     // unsharded runs: no windows, parity 0, stamp 1
     p.xpar = x->epoch & 1; p.stamp = x->epoch + 1; p.loopback = x->loopback ? 1u : 0u;
-    p.win_cap = x->win_cap; p.win_data = x->peer_data[p.xpar]; p.send_count = x->send_count; p.peer_ctrl = x->peer_ctrl;
+    snd.win_cap = x->win_cap; snd.win_data = x->peer_data[p.xpar]; snd.send_count = x->send_count; p.peer_ctrl = x->peer_ctrl;
     p.fuse_publish = (!h->byz_on && !h->sw.no_fuse) ? 1u : 0u;
   }
-  p.shard_inv = (u32)(0x100000000ull / h->shard_size); p.xcap = p.world > 1 ? XW_TOTAL / (p.world - 1) : 0u;
+  p.xcap = snd.world > 1 ? XW_TOTAL / (snd.world - 1) : 0u;
   if (h->gate_on) {                                // convergence gate: the first kernel of the tick evaluates the row of tick t-1
     const u64* grow = h->xc ? h->xc->grow : h->d_trace;            // global rows: the device sums them when sharded
     Gate& g = p.gate;
@@ -468,8 +468,7 @@ void launch_user_events(serfsim* h, const TickParams& p) {
   u.ltime = h->ue->ltime; u.node_state = h->d_node; u.busy = h->d_busy; u.row_ptr = h->d_rowptr; u.col = h->d_col;
   u.ev_node = h->d_ev_node; u.ev_op = h->d_ev_op; u.ev_slot = h->d_ev_slot;
   u.row = p.row; u.totals = h->ue->totals; u.overflow = h->d_overflow; u.sched = h->d_sched;
-  u.world = p.world; u.rank = p.rank; u.shard_size = h->shard_size; u.win_cap = p.win_cap;
-  u.win_data = p.win_data; u.send_count = p.send_count;
+  u.snd = p.snd;
   u.gate = p.gate; u.gate.evaluate = 1u;
   launch_uevent(u, h->cfg.trace != 0, h->stream);
   h->last_launches++;
@@ -517,8 +516,7 @@ void launch_injectors(serfsim* h, const TickParams& p) {
   b.seed_lo = p.seed_lo; b.seed_hi = p.seed_hi; b.delta = h->byz_delta; b.ids = h->byz->ids; b.rec = h->d_rec; b.node_state = h->d_node;
   b.row_ptr = h->d_rowptr; b.col = h->d_col; b.inbox_wr = h->d_inbox[t & 1]; b.hot_wr = h->d_hot[t & 1]; b.kinds_cur = p.kinds_cur;
   b.anomaly = h->byz->anomaly; b.totals = h->byz->totals;
-  b.n_local = h->count; b.world = p.world; b.rank = p.rank; b.shard_size = h->shard_size; b.win_cap = p.win_cap;
-  b.win_data = p.win_data; b.send_count = p.send_count; b.overflow = h->d_overflow; b.gate = p.gate.ctl;
+  b.n_local = h->count; b.snd = p.snd; b.overflow = h->d_overflow; b.gate = p.gate.ctl;
   launch_byz(b, h->stream);
   h->last_launches++;
 }
@@ -533,16 +531,16 @@ int launch_exchange(serfsim* h, const TickParams& p) {
     CU(cudaEventRecord(x.mid_ev[t], h->stream));
   }
   PublishParams pb{};
-  pb.world = p.world; pb.rank = p.rank; pb.stamp = p.stamp; pb.xpar = xpar; pb.send_count = x.send_count; pb.peer_ctrl = x.peer_ctrl;
+  pb.world = p.snd.world; pb.rank = p.snd.rank; pb.stamp = p.stamp; pb.xpar = xpar; pb.send_count = x.send_count; pb.peer_ctrl = x.peer_ctrl;
   pb.row = p.row; pb.gate = p.gate.ctl; pb.sched = h->d_sched; pb.loopback = p.loopback;
   if (!p.fuse_publish) { launch_publish(pb, h->stream); h->last_launches++; }
   DrainParams d{};
-  d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.world; d.rank = p.rank; d.win_cap = x.win_cap; d.stamp = p.stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
-  d.win_data = x.win_data[xpar]; d.ctrl = x.ctrl + xpar * 16; d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
-  d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = h->shard_size; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = x.peer_anomaly;
+  d.n_local = h->count; d.stride = h->stride; d.R = h->R; d.world = p.snd.world; d.rank = p.snd.rank; d.win_cap = x.win_cap; d.stamp = p.stamp; d.n_tiles = h->n_tiles; d.kinds_prev = p.kinds_prev;
+  d.win_data = x.win_data[xpar]; d.counts = ctrl_counts(x.ctrl, xpar); d.flags = ctrl_flags(x.ctrl, xpar); d.inbox_wr = h->d_inbox[t & 1]; d.hot_wr = h->d_hot[t & 1]; d.kinds_cur = p.kinds_cur; d.overflow = h->d_overflow;
+  d.byz_on = h->byz_on ? 1u : 0u; d.byz_delta = h->byz_delta; d.shard_size = p.snd.shard_size; d.shard_inv = p.snd.shard_inv; d.rec = h->d_rec; d.node_state = h->d_node; d.peer_anomaly = x.peer_anomaly;
   d.ue_n = h->ue_table.n; d.ue_inbox_wr = h->ue_table.n ? h->ue->inbox[t & 1].get() : nullptr; d.ue_ltime = h->ue ? h->ue->ltime.get() : nullptr;
   d.my_row = p.row; d.grow = x.grow + (size_t)t * ROW_FIELDS; d.gate = p.gate.ctl;
-  d.sums = reinterpret_cast<const u64*>(reinterpret_cast<const unsigned char*>(x.ctrl.get()) + CTRL_SUMS_OFF) + (size_t)xpar * 8 * CTRL_FIELDS;
+  d.sums = ctrl_sums(x.ctrl, xpar);
   d.sched = h->d_sched; d.sched_rw = h->d_sched; d.host_idle_until = h->d_pin_ctl + 2; d.tick = t; d.sleep_on = p.sleep_on;
   launch_drain(d, h->stream);
   h->last_launches += 1;
@@ -868,10 +866,10 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   std::unique_ptr<serfsim> h(new serfsim());
   h->cfg = *cfg; h->N = cfg->n_nodes; h->R = cfg->slots;
   h->shard_size = (h->N + cfg->world_size - 1) / cfg->world_size;
-  h->first = std::min<u64>((u64)h->shard_size * cfg->rank, h->N);
-  h->count = (u32)std::min<u64>(h->shard_size, (u64)h->N - h->first);
+  const ShardSpan span = shard_span((u32)cfg->rank, h->shard_size, h->N);
+  h->first = span.first; h->count = span.count; h->stride = span.stride;
   if (h->count == 0) return fail(SERFSIM_E_INVAL, "empty shard");
-  if (h->shard_size >= (1u << 26)) return fail(SERFSIM_E_INVAL, "shard larger than 2^26 nodes");
+  if (h->shard_size >= (1u << WIN_DST_BITS)) return fail(SERFSIM_E_INVAL, "shard larger than 2^26 nodes");
   h->rules.limit = (u32)retransmit_limit(cfg->retransmit_mult, h->N);      // 1..255: checked above
   auto tab = suspicion_table(cfg->suspicion_mult, cfg->suspicion_max_timeout_mult, cfg->probe_interval_ticks ? cfg->probe_interval_ticks : 1, cfg->gossip_interval_ms, h->N);
   h->rules.k = (u32)tab.size() - 1;
@@ -881,7 +879,6 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
 
   CU(h->stream.create());
   CU(h->ev0.create()); CU(h->ev1.create());
-  h->stride = plane_stride(h->count);
   h->n_tiles = h->stride >> TILE_SHIFT;
   const size_t planes = (size_t)h->R * h->stride;
   CU(h->d_rec.alloc(2 * planes)); CU(h->d_rec.fill(0, h->stream));
@@ -918,7 +915,7 @@ int serfsim_create(const serfsim_config_t* cfg, serfsim_t** out) {
   }
   if (cfg->world_size > 1) {
     // receive windows: one segment per peer; expected entries per tick and pair ≈ shard · fanout · R · kinds / world
-    if (cfg->world_size > MAX_WORLD) return fail(SERFSIM_E_INVAL, "world_size > 8");
+    if (cfg->world_size > (int)MAX_WORLD) return fail(SERFSIM_E_INVAL, "world_size > 8");
     serfsim::Exchange x;
     // … plus what a warp of the tick kernel (TILE threads) can leave unfilled in a peer's window: its reservation ahead and a partial block
     const double pad = (double)std::max(h->grid, h->grid_sv) * (TILE / 32) * (XW_RESERVE_MAX + XW_FLUSH);   // (the single-view kernel of a multi-slot run has the larger grid)
@@ -1526,11 +1523,11 @@ int serfsim_comm_loopback(serfsim_t* h) {
   if (h->cfg.rank != 0) return fail(SERFSIM_E_INVAL, "loopback: create the handle as rank 0");
   if (h->cfg.push_pull_interval_ticks > 0 || h->byz_on || h->ue_table.n) return fail(SERFSIM_E_INVAL, "loopback profiles the membership path only");
   serfsim::Exchange& x = *h->xc;
-  // entries for shard s are written at win_data[s][rank·win_cap + g]: with rank 0 the window of "peer" s is my own segment s
+  // entries for shard s go to segment `rank` of the window of "peer" s: with rank 0 that is my own segment s
   PeerTables t;
   for (int r = 0; r < h->cfg.world_size; ++r) {
     t.ctrl[r] = x.ctrl; t.anomaly[r] = h->byz->anomaly;
-    for (int par = 0; par < 2; ++par) t.data[par][r] = x.win_data[par] + (size_t)r * x.win_cap;
+    for (int par = 0; par < 2; ++par) t.data[par][r] = win_segment(x.win_data[par], r, x.win_cap);
   }
   if (int rc = install_peers(h, t)) return rc;
   x.barrier = [](void*) {}; x.allreduce = [](void*, uint64_t*, uint32_t) {};

@@ -170,19 +170,10 @@ __device__ __forceinline__ u64 warp_sum64(u64 v) {
 // with a warp-aggregated shared-memory atomic and a buffer that holds at least 32 entries is copied into the peer's
 // window by its own warp — 256+ contiguous bytes over NVLink, one global counter atomic per flush, no CTA barrier
 // anywhere (a per-tile CTA-wide flush cost four barriers per tile and made every warp wait for the slowest one).
-constexpr u32 MAX_WORLD = 8;
 struct XStage { u64 buf[(BLOCK / 32) * XW_TOTAL]; u32 cnt[BLOCK / 32][MAX_WORLD]; };
-// (no integer division on the send path: the sharded kernel issues on every cycle it can — 2.4× the instructions of the unsharded one —
-// and `x / runtime value` is ≈ 25 of them; capacity and reciprocal come with the parameters)
-__device__ __forceinline__ u32 xcap(const TickParams& p) { return p.xcap; }
-__device__ __forceinline__ u32 xseg(const TickParams& p, u32 shard) { return (shard - (shard > p.rank ? 1u : 0u)) * p.xcap; }
-__device__ __forceinline__ u32 shard_of(const TickParams& p, u32 dst, u32& dloc) {
-  u32 q = mulhi32(dst, p.shard_inv);           // floor(dst / shard_size) or one less
-  u32 r = dst - q * p.shard_size;
-  if (r >= p.shard_size) { ++q; r -= p.shard_size; }
-  dloc = r;
-  return q;
-}
+// (no integer division on the send path: the sharded kernel issues on every cycle it can — 2.4× the instructions of the unsharded one;
+// the staging capacity comes with the parameters, and shard_of uses the reciprocal)
+__device__ __forceinline__ u32 xseg(const TickParams& p, u32 shard) { return (shard - (shard > p.snd.rank ? 1u : 0u)) * p.xcap; }
 
 // held: what the sender read from the destination word earlier in this launch (0: nothing read).  The words of the plane only
 // grow during a launch (RED.MAX is the only write to the planes a launch sends into), so held ≥ val1 means the word already is,
@@ -195,9 +186,9 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
     else SFS_PROBE(22);
     if (mark) { p.hot_wr[dl >> TILE_SHIFT] = 1; SFS_PROBE(26); }   // sparse ticks only: tell the next tick which tiles received something
   } else {
-    u32 dloc;
-    const u32 shard = shard_of(p, dst, dloc);
-    const u64 e = win_entry(val1, s + p.sv_wshift, kind, dloc);   // (a single-view launch numbers its view 0: the entry carries the real one)
+    const ShardIdx t = shard_of(dst, p.snd.shard_size, p.snd.shard_inv);
+    const u32 shard = t.shard;
+    const u64 e = win_entry(val1, s + p.sv_wshift, kind, t.local);   // (a single-view launch numbers its view 0: the entry carries the real one)
     // warp-aggregated append: the lanes of this call that target the same shard reserve their slots with ONE
     // shared-memory atomic on the warp's own counter (divergent callers of the same warp may interleave: keep it atomic)
 #ifdef SFS_XSTAGE_MATCH                           // A/B: one shared atomic per distinct shard of the call (match_any + leader + shuffle)
@@ -211,10 +202,10 @@ __device__ __forceinline__ void deliver(const TickParams& p, XStage* xs, u32* pl
     const u32 wid = threadIdx.x >> 5;
     const u32 pos = atomicAdd(&xs->cnt[wid][shard], 1u);
 #endif
-    if (pos < xcap(p)) {
+    if (pos < p.xcap) {
       xs->buf[wid * XW_TOTAL + xseg(p, shard) + pos] = e;
     } else {                                   // buffer full: write this one straight through
-      win_append<1>(p, shard, {e});
+      win_append<1>(p.snd, p.overflow, shard, {e});
     }
   }
 }
@@ -244,33 +235,34 @@ __device__ __forceinline__ void send_deduped(const TickParams& p, u32* plane, co
 // is all zeros again before it is written next.  force = false: whole blocks only; force = true (end of the kernel): everything.
 __device__ __forceinline__ bool flush_xwarp(const TickParams& p, XStage* xs, bool force, u32& resv, u32& rlen) {
   const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const Sender& x = p.snd;
   __syncwarp();
   bool wrote = false;
   u32 want = 0;                                // this lane's peer: entries to reserve for the next flush
   // peers whose buffer holds a whole block (anything, when forced): lane s looks at peer s, one vote, then only those are visited
-  const u32 mine = lane < p.world ? xs->cnt[wid][lane] : 0u;
-  u32 ready = __ballot_sync(0xffffffffu, lane != p.rank && (force ? mine != 0 : mine >= XW_FLUSH));
+  const u32 mine = lane < x.world ? xs->cnt[wid][lane] : 0u;
+  u32 ready = __ballot_sync(0xffffffffu, lane != x.rank && (force ? mine != 0 : mine >= XW_FLUSH));
   while (ready) {
     const u32 sh = (u32)__ffs((int)ready) - 1u;
     ready &= ready - 1u;
     const u32 staged = __shfl_sync(0xffffffffu, mine, sh);
-    if (staged > xcap(p)) wrote = true;        // the excess went straight through
-    const u32 n = min(staged, xcap(p));
+    if (staged > p.xcap) wrote = true;        // the excess went straight through
+    const u32 n = min(staged, p.xcap);
     const u32 m = force ? n : (n & ~(XW_FLUSH - 1u));          // entries to write now
     u64* src = xs->buf + wid * XW_TOTAL + xseg(p, sh);
-    u64* dst = p.win_data[sh] + (size_t)p.rank * p.win_cap;
+    u64* dst = win_segment(x.win_data[sh], x.rank, x.win_cap);
     const u32 base = __shfl_sync(0xffffffffu, resv, sh), avail = __shfl_sync(0xffffffffu, rlen, sh);
     const u32 take = min(m, avail);
     for (u32 i = lane; i < take; i += 32) {
-      if (base + i < p.win_cap) dst[base + i] = src[i];
+      if (base + i < x.win_cap) dst[base + i] = src[i];
       else *p.overflow = 2;
     }
     if (m > take) {                            // not (enough) reserved ahead: take the rest now
       u32 b2 = 0;
-      if (lane == sh) b2 = atomicAdd(p.send_count + sh, m - take);
+      if (lane == sh) b2 = atomicAdd(x.send_count + sh, m - take);
       b2 = __shfl_sync(0xffffffffu, b2, sh);
       for (u32 i = lane; i < m - take; i += 32) {
-        if (b2 + i < p.win_cap) dst[b2 + i] = src[take + i];
+        if (b2 + i < x.win_cap) dst[b2 + i] = src[take + i];
         else *p.overflow = 2;
       }
     }
@@ -284,7 +276,7 @@ __device__ __forceinline__ bool flush_xwarp(const TickParams& p, XStage* xs, boo
     if (lane == 0) xs->cnt[wid][sh] = rem;
   }
   // reservations for the next flush: issued last, consumed by the shuffles of the NEXT call
-  if (!force && want && rlen == 0) { resv = atomicAdd(p.send_count + lane, want); rlen = want; }
+  if (!force && want && rlen == 0) { resv = atomicAdd(x.send_count + lane, want); rlen = want; }
   __syncwarp();
   return wrote;
 }
@@ -746,14 +738,14 @@ __device__ __forceinline__ void publish_to_peer(u32 r, u32 world, u32 rank, u32 
                                                 const volatile u64* row, const volatile u32* sched) {
   if (r >= world || r == rank) return;
   const u32 me = loopback ? r : rank;                       // the slot this rank owns in the peer's control block
-  u32* ctrl = peer_ctrl[r] + xpar * 16;
-  ctrl[me] = send_count[r];
-  u64* sums = reinterpret_cast<u64*>(reinterpret_cast<unsigned char*>(peer_ctrl[r]) + CTRL_SUMS_OFF) + ((size_t)xpar * 8 + me) * CTRL_FIELDS;
+  u32* const ctrl = peer_ctrl[r];
+  ctrl_counts(ctrl, xpar)[me] = send_count[r];
+  u64* sums = ctrl_sums(ctrl, xpar)[me];
 #pragma unroll
   for (int i = 0; i < ROW_FIELDS; ++i) sums[i] = row[i];              // this rank's counters of the tick: every rank sums them on the device
-  sums[ROW_FIELDS] = sched[SCHED_LOCAL_QUIET]; sums[ROW_FIELDS + 1] = sched[SCHED_LOCAL_UNTIL]; sums[ROW_FIELDS + 2] = sched[SCHED_VIEWS_NEW];
+  sums[CTRL_QUIET] = sched[SCHED_LOCAL_QUIET]; sums[CTRL_UNTIL] = sched[SCHED_LOCAL_UNTIL]; sums[CTRL_VIEWS] = sched[SCHED_VIEWS_NEW];
   __threadfence_system();
-  st_release_sys(ctrl + 8 + me, stamp);
+  st_release_sys(ctrl_flags(ctrl, xpar) + me, stamp);
   send_count[r] = 0;
 }
 
@@ -828,7 +820,7 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
   }
   if (threadIdx.x == 0) {
     row[ROW_PENDING] = row[ROW_PENDING] + suspects;                            // pending = awake views counted above + sleeping Suspect views
-    if (p.world == 1) {
+    if (p.snd.world == 1) {
       sched[SCHED_IDLE_UNTIL] = until;
       if (p.host_idle_until) *p.host_idle_until = until;
     } else {
@@ -842,11 +834,11 @@ __device__ __forceinline__ void finish_tick(const TickParams& p, const Counters&
     const u32 sv_base = views_of_tick(sched, p.tick);   // what this kernel's CTAs read when they started (nobody else writes these words)
     sched[SCHED_VIEWS_OLD] = sv_base; sched[SCHED_VIEWS_NEW] = sched[SCHED_VIEWS_NEXT] | sv_next; sched[SCHED_VIEWS_FROM] = p.tick + 1; sched[SCHED_VIEWS_NEXT] = 0;   // the views with business in the next tick (kernels that follow in this tick — anti-entropy, drain — add to it)
   }
-  if (p.world > 1 && p.fuse_publish) {
+  if (p.snd.world > 1 && p.fuse_publish) {
     // every CTA fenced its peer-window stores (system scope) before it took its ticket; this one saw all tickets
     __syncthreads();
     __threadfence();
-    publish_to_peer(threadIdx.x, p.world, p.rank, p.xpar, p.stamp, p.loopback, p.peer_ctrl, p.send_count, row, sched);
+    publish_to_peer(threadIdx.x, p.snd.world, p.snd.rank, p.xpar, p.stamp, p.loopback, p.peer_ctrl, p.snd.send_count, row, sched);
   }
 }
 
@@ -879,7 +871,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
     const bool single = views == (1u << p.sv_slot);        // exactly the one view the single-view launch was set up for
     if (p.sv_mode == SV_SINGLE) { if (!single) return; SFS_PROBE(21); }
     else if (p.sv_mode == SV_GENERAL && single) return;
-    if (p.sv_mode == SV_CHECK && (single || p.world == 1)) sv_views = views;   // checked where the single-view kernel or the passes would have run
+    if (p.sv_mode == SV_CHECK && (single || p.snd.world == 1)) sv_views = views;   // checked where the single-view kernel or the passes would have run
   }
   if (threadIdx.x == 0) dsusp_s = 0;                       // ordered before its first use by the barrier after the tile scan
   Counters c = {};
@@ -909,7 +901,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
 
   const u32 tile0 = blockIdx.x * p.tiles_per_cta;
   const u32 ntile = tile0 < p.n_tiles ? min(p.tiles_per_cta, p.n_tiles - tile0) : 0;
-  if (SHARDED && saturated && ntile && (u32)lane < p.world && (u32)lane != p.rank) { resv = atomicAdd(p.send_count + lane, XW_FLUSH); rlen = XW_FLUSH; }   // every warp will send to every peer
+  if (SHARDED && saturated && ntile && (u32)lane < p.snd.world && (u32)lane != p.snd.rank) { resv = atomicAdd(p.snd.send_count + lane, XW_FLUSH); rlen = XW_FLUSH; }   // every warp will send to every peer
   if (PASS && p.sv_slot != 0) tile_decisions(p, hot_s, tile0, ntile, p.sv_slot + 1u == p.sv_R, work); else scan_tiles(p, hot_s, tile0, ntile, all_hot, PASS);
   __syncthreads();
   if (PASS && !work && p.sv_slot + 1u < p.sv_R) return;   // the first pass without business has made the tiles' decisions
@@ -1186,11 +1178,12 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
     const u64* part_node = snap_node;
     const uint4* part_rec = snap_rec;
     u32 part_stride = p.stride;
-    if (p.world > 1) {
-      const u32 shard = u / p.shard_size;
-      ul = u - shard * p.shard_size;
+    u32 shard = 0;
+    if (p.snd.world > 1) {
+      const ShardIdx t = shard_of(u, p.snd.shard_size, p.snd.shard_inv);
+      shard = t.shard; ul = t.local;
       part_node = p.snap_node_peer[shard]; part_rec = p.snap_rec_peer[shard];
-      part_stride = plane_stride(min(p.shard_size, p.n_global - shard * p.shard_size));
+      part_stride = shard_span(shard, p.snd.shard_size, p.n_global).stride;
     }
     const u64 nu = part_node[ul];
     if (!nw_up(nu)) continue;
@@ -1243,7 +1236,7 @@ __global__ void __launch_bounds__(BLOCK) pushpull_kernel(const __grid_constant__
       if (r.inc >= INC_LIMIT) *p.overflow = 1;
     }
     if (p.ue_table.n) {                                        // the partner's event clock and ring (a snapshot, like its records)
-      const uint4 pw = (p.world > 1 ? p.ue_snap_peer[u / p.shard_size] : p.ue_snap)[ul];
+      const uint4 pw = (p.snd.world > 1 ? p.ue_snap_peer[shard] : p.ue_snap)[ul];
       const uint4 w0 = p.ue_state[vl];
       UeRec er;
       ue_unpack(w0, er);
@@ -1294,13 +1287,13 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
   if (p.gate && *p.gate) return;
   if (threadIdx.x < p.world && threadIdx.x != p.rank) {
     u32 f;
-    do { f = ld_acquire_sys(p.ctrl + 8 + threadIdx.x); } while (f != p.stamp);
+    do { f = ld_acquire_sys(p.flags + threadIdx.x); } while (f != p.stamp);
   }
   __syncthreads();
   // global trace row of this tick: my counters + the rows the peers published with their flags (acquired above)
   if (blockIdx.x == 0 && threadIdx.x < ROW_FIELDS) {
     u64 s = p.my_row[threadIdx.x];
-    for (u32 src = 0; src < p.world; ++src) if (src != p.rank) s += __ldcg(p.sums + (size_t)src * CTRL_FIELDS + threadIdx.x);
+    for (u32 src = 0; src < p.world; ++src) if (src != p.rank) s += __ldcg(&p.sums[src][threadIdx.x]);
     p.grow[threadIdx.x] = s;
   }
   // The ranks' scheduler verdicts: the cluster sleeps iff every rank is quiet, until the earliest of their deadlines.  Every rank
@@ -1312,12 +1305,12 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
     u32 until = p.sched[SCHED_LOCAL_UNTIL];
     for (u32 src = 0; src < p.world; ++src) {
       if (src == p.rank) continue;
-      quiet = quiet && __ldcg(p.sums + (size_t)src * CTRL_FIELDS + ROW_FIELDS) != 0;
-      until = min(until, (u32)__ldcg(p.sums + (size_t)src * CTRL_FIELDS + ROW_FIELDS + 1));
+      quiet = quiet && __ldcg(&p.sums[src][CTRL_QUIET]) != 0;
+      until = min(until, (u32)__ldcg(&p.sums[src][CTRL_UNTIL]));
     }
     if (p.host_idle_until) *p.host_idle_until = quiet ? max(until, p.tick + 1) : p.tick + 1;
     u32 views = 0;                                        // views with business in the next tick: anywhere in the cluster (their mail crosses shards)
-    for (u32 src = 0; src < p.world; ++src) if (src != p.rank) views |= (u32)__ldcg(p.sums + (size_t)src * CTRL_FIELDS + ROW_FIELDS + 2);
+    for (u32 src = 0; src < p.world; ++src) if (src != p.rank) views |= (u32)__ldcg(&p.sums[src][CTRL_VIEWS]);
     if (views) atomicOr(p.sched_rw + SCHED_VIEWS_NEW, views);
   }
   // the tick kernel's dense / sparse decision of this tick: in a dense tick the next tick processes every
@@ -1326,8 +1319,8 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
   u32 seen = 0;                                 // kinds this thread folded (bit per kind)
   for (u32 src = 0; src < p.world; ++src) {
     if (src == p.rank) continue;
-    const u32 n = min(p.ctrl[src], p.win_cap);
-    u64* w = p.win_data + (size_t)src * p.win_cap;
+    const u32 n = min(p.counts[src], p.win_cap);
+    u64* w = win_segment(p.win_data, src, p.win_cap);
     for (u32 i = blockIdx.x * BLOCK + threadIdx.x; i < n; i += gridDim.x * BLOCK) {
       const u64 e = __ldcg(w + i);
       if (e == 0) continue;                          // padding of a partly filled block (a real entry has value + 1 > 0 in its high word)
@@ -1350,7 +1343,7 @@ __global__ void __launch_bounds__(BLOCK) drain_kernel(const __grid_constant__ Dr
           if (nw_up(p.node_state[dl])) {
             Rec q;
             unpack(load_rec(p.rec, (size_t)s * p.stride + dl), q);
-            if (byz_anomalous(q, be, p.byz_delta)) { const u32 sh = src / p.shard_size; p.peer_anomaly[sh][src - sh * p.shard_size] = 1; }
+            if (byz_anomalous(q, be, p.byz_delta)) { const ShardIdx t = shard_of(src, p.shard_size, p.shard_inv); p.peer_anomaly[t.shard][t.local] = 1; }
           }
         }
       } else if (dl < p.n_local && kind == KIND_EXTRA && s < p.ue_n && val1) {   // user event s arrived: one bit, and the time its origin stamped
@@ -1387,8 +1380,8 @@ __global__ void __launch_bounds__(BLOCK) clear_windows_kernel(const __grid_const
   if (p.gate && *p.gate) return;
   for (u32 src = 0; src < p.world; ++src) {
     if (src == p.rank) continue;
-    const u32 n = min(p.ctrl[src], p.win_cap);
-    u64* w = p.win_data + (size_t)src * p.win_cap;
+    const u32 n = min(p.counts[src], p.win_cap);
+    u64* w = win_segment(p.win_data, src, p.win_cap);
     for (u32 i = blockIdx.x * BLOCK + threadIdx.x; i < n; i += gridDim.x * BLOCK) w[i] = 0;
   }
 }
@@ -1545,7 +1538,7 @@ static void launch_tick_tma(const TickParams& p, int grid, bool barsync, cudaStr
 
 template <bool TRACE, int FMAX>
 static void launch_tick_v(const TickParams& p, int grid, int ctas_per_sm, bool tma_sync, cudaStream_t st) {
-  const bool sharded = p.world > 1, r1 = p.R == 1;
+  const bool sharded = p.snd.world > 1, r1 = p.R == 1;
 #ifndef SERFSIM_EMU
   if (r1 && p.stage_col_bytes && !sharded) { // single-slot, single-GPU run whose tiles fit a shared-memory stage: TMA pipeline
     launch_tick_tma<TRACE, FMAX, false>(p, grid, tma_sync, st);

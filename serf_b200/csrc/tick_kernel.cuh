@@ -40,26 +40,75 @@ enum : u32 { ROW_PACKETS = 0, ROW_EDGES = 1, ROW_MESSAGES = 2, ROW_CHANGED = 3, 
 SFS_HD u32 sent_messages(const u32* kinds) { return kinds[KIND_LEAVE] + kinds[KIND_JOIN] + kinds[KIND_ML]; }
 SFS_HD bool dense_tick(u32 prev_msgs, u32 n_tiles) { return prev_msgs >= (n_tiles >> 1) + 1; }
 
-// Cross-shard window entry (8 B): value + 1 << 32 | view << 28 | kind << 26 | destination (26 bits, local to its shard).
+// ---- The cross-shard exchange of a sharded run (world > 1) ----
+// Shards: rank r owns the global ids [r·shard_size, (r+1)·shard_size) that are < n_global.
+constexpr u32 MAX_WORLD = 8;                 // ranks of a sharded run
+// A target's shard without a division (`x / runtime value` is ≈ 25 instructions on the send path): q = mulhi(id, shard_inv) is
+// floor(id / shard_size) or one less with shard_inv = floor(2^32 / shard_size), and with 2^32 - 1 for shard_size 1 (2^32 has no u32).
+SFS_HD u32 shard_recip(u32 shard_size) { return shard_size > 1 ? (u32)(0x100000000ull / shard_size) : 0xffffffffu; }
+struct ShardIdx { u32 shard, local; };
+SFS_HD ShardIdx shard_of(u32 id, u32 shard_size, u32 shard_inv) {
+  ShardIdx x;
+  x.shard = mulhi32(id, shard_inv);
+  x.local = id - x.shard * shard_size;
+  if (x.local >= shard_size) { ++x.shard; x.local -= shard_size; }
+  return x;
+}
+// Shard r: its first global id, its node count (the last shard may be short) and the stride of its per-slot planes
+struct ShardSpan { u32 first, count, stride; };
+SFS_HD ShardSpan shard_span(u32 r, u32 shard_size, u32 n_global) {
+  const u64 f = (u64)shard_size * r;
+  const u32 first = f < n_global ? (u32)f : n_global, rest = n_global - first;
+  const u32 count = rest < shard_size ? rest : shard_size;
+  return {first, count, plane_stride(count)};
+}
+
+// Window entry (8 B): value + 1 << 32 | view << 28 | kind << 26 | destination (WIN_DST_BITS, local to its shard).
 // Kind 3 (KIND_EXTRA) is a user event (view = the event) or the annotation of an injector triple (ByzParams).
 constexpr u32 KIND_EXTRA = 3;
-SFS_HD u64 win_entry(u32 val1, u32 s, u32 kind, u32 dloc) { return ((u64)val1 << 32) | ((u64)s << 28) | ((u64)kind << 26) | dloc; }
+constexpr u32 WIN_DST_BITS = 26;             // a shard holds fewer than 2^WIN_DST_BITS nodes
+constexpr u32 BYZ_FLAG = 1u << (WIN_DST_BITS - 1);   // injector entries: the top bit of the destination (their shards hold fewer than BYZ_FLAG nodes)
+SFS_HD u64 win_entry(u32 val1, u32 s, u32 kind, u32 dloc) { return ((u64)val1 << 32) | ((u64)s << 28) | ((u64)kind << WIN_DST_BITS) | dloc; }
 SFS_HD u32 win_val1(u64 e) { return (u32)(e >> 32); }
 SFS_HD u32 win_slot(u64 e) { return (u32)(e >> 28) & 15; }
-SFS_HD u32 win_kind(u64 e) { return (u32)(e >> 26) & 3; }
-SFS_HD u32 win_dst(u64 e) { return (u32)e & ((1u << 26) - 1); }
-// Append N entries to this rank's segment of peer `shard`'s window (P: a parameter block with the window fields); a full
-// window raises overflow 2.
-template <u32 N, class P>
-__device__ __forceinline__ void win_append(const P& p, u32 shard, const u64 (&e)[N]) {
-  const u32 g = atomicAdd(p.send_count + shard, N);
-  if (g + (N - 1) < p.win_cap) {
+SFS_HD u32 win_kind(u64 e) { return (u32)(e >> WIN_DST_BITS) & 3; }
+SFS_HD u32 win_dst(u64 e) { return (u32)e & ((1u << WIN_DST_BITS) - 1); }
+// Every rank owns one receive window per exchange parity, [world][win_cap] entries: rank r writes segment r of each peer's window.
+SFS_HD u64* win_segment(u64* window, u32 r, u32 win_cap) { return window + (size_t)r * win_cap; }
+
+// What a kernel that sends into the peers' windows reads (TickParams, UeParams, ByzParams); world = 1 and no windows when unsharded.
+struct Sender {
+  u32 world, rank, shard_size, win_cap;
+  u64* const* win_data;       // [world] peer windows of this exchange parity
+  u32* send_count;            // [world] entries written so far into each peer's window (local counters, shared by the tick's kernels)
+  u32 shard_inv;              // shard_recip(shard_size)
+};
+// Append N entries to this rank's segment of peer `shard`'s window; a full window raises overflow 2.
+template <u32 N>
+__device__ __forceinline__ void win_append(const Sender& x, u32* overflow, u32 shard, const u64 (&e)[N]) {
+  const u32 g = atomicAdd(x.send_count + shard, N);
+  if (g + (N - 1) < x.win_cap) {
+    u64* const seg = win_segment(x.win_data[shard], x.rank, x.win_cap);
 #pragma unroll
-    for (u32 i = 0; i < N; ++i) p.win_data[shard][(size_t)p.rank * p.win_cap + g + i] = e[i];
+    for (u32 i = 0; i < N; ++i) seg[g + i] = e[i];
   } else {
-    *p.overflow = 2;
+    *overflow = 2;
   }
 }
+
+// Control block of a rank (one allocation, mapped into every peer), per exchange parity: the entry counts and release flags the peers
+// write, and the trace row each peer published with its flag (the device-side sum of the per-tick counters), then its scheduler verdict.
+constexpr u32 CTRL_QUIET = ROW_FIELDS, CTRL_UNTIL = ROW_FIELDS + 1, CTRL_VIEWS = ROW_FIELDS + 2;   // quiet (0 / 1), sleep until, views with business next tick
+constexpr u32 CTRL_FIELDS = ROW_FIELDS + 3;
+typedef u64 CtrlRow[CTRL_FIELDS];
+struct CtrlBlock {
+  struct { u32 counts[MAX_WORLD], flags[MAX_WORLD]; } par[2];   // [parity][source rank]
+  CtrlRow sums[2][MAX_WORLD];                                  // [parity][source rank]
+};
+constexpr size_t CTRL_BYTES = sizeof(CtrlBlock);
+SFS_HD u32* ctrl_counts(u32* ctrl, u32 par) { return reinterpret_cast<CtrlBlock*>(ctrl)->par[par].counts; }
+SFS_HD u32* ctrl_flags(u32* ctrl, u32 par) { return reinterpret_cast<CtrlBlock*>(ctrl)->par[par].flags; }
+SFS_HD CtrlRow* ctrl_sums(u32* ctrl, u32 par) { return reinterpret_cast<CtrlBlock*>(ctrl)->sums[par]; }
 
 // Cross-shard staging of the tick kernel: staged entries per warp (3 KB), split evenly over the world-1 peers (world 8: 56 each)
 // (TickParams::xcap); a full warp-wide store flushes; at most XW_RESERVE_MAX entries reserved ahead per warp and peer.
@@ -135,9 +184,7 @@ struct TickParams {
   // cross-shard exchange (world_size > 1): every rank owns one receive window per peer (mapped into the
   // peers with CUDA IPC); the tick kernel stages cross-shard entries per destination shard in shared memory
   // and writes them into the peer's window with coalesced stores over NVLink.
-  u32 world, rank, shard_size, win_cap;
-  u64* const* win_data;       // [world] peer windows of this exchange parity; my segment starts at rank·win_cap
-  u32* send_count;            // [world] entries written so far into each peer's window (local counters)
+  Sender snd;
   // sharded push-pull rounds: every rank's end-of-tick snapshot, indexed by shard (null when world == 1).  New members go
   // at the end: the tick kernels do not read them and keep their parameter offsets (and their SASS) unchanged.
   const uint4* const* snap_rec_peer; const u64* const* snap_node_peer;
@@ -161,7 +208,7 @@ struct TickParams {
   // sharded runs without injectors: the tick's LAST CTA also publishes (counts, row, verdict, release flag → every peer's control
   // block): one launch less per tick.  With injectors their kernel still writes windows after this one, and publish_kernel follows it.
   u32* const* peer_ctrl; u32 stamp, xpar, loopback, fuse_publish;
-  u32 shard_inv, xcap;        // floor(2^32 / shard_size) (a remote target's shard without a division); staged entries per warp and peer
+  u32 xcap;                   // staged entries per warp and peer
   u32 sv_wshift;              // single-view launch: its view's bit in the watch masks (0 in every other launch)
   u32 sv_mode, views_host, sv_slot, sv_R;    // single-view ticks (SV_*, below): sv_slot = the view the single-view launch works on, sv_R = number of views of the run
   u32 ahead;                  // multi-slot runs: 1 = saturated ticks request node word, peers and the probable first view's record one tile ahead; 2 = every tick (tests); 0 = off (SERFSIM_AHEAD)
@@ -214,12 +261,6 @@ __device__ __forceinline__ u32 host_op_of(const P& p, u32 v, u32& op_slot) {
   return 0;
 }
 
-// Control block of a rank (one allocation, mapped into every peer): per exchange parity the entry counts and epoch flags
-// the peers write, then the peers' trace rows of that tick (the device-side sum of the per-tick counters).
-constexpr u32 CTRL_U32 = 2 * 16;                        // [parity][ counts[8] | flags[8] ]
-constexpr u32 CTRL_SUMS_OFF = CTRL_U32 * 4;             // byte offset of u64 sums[2][8][CTRL_FIELDS]  ([parity][source rank][field])
-constexpr u32 CTRL_FIELDS = 11;                         // the 8 trace-row fields, then the rank's scheduler verdict: 8 = quiet (0 / 1), 9 = sleep until, 10 = views with business in the next tick
-constexpr size_t CTRL_BYTES = CTRL_SUMS_OFF + 2 * 8 * CTRL_FIELDS * sizeof(u64);
 struct PublishParams {        // after the tick kernel: tell every peer how much was written and this rank's row, then raise its flag
   u32 world, rank, stamp, xpar;
   u32* send_count;            // [world] local, reset here
@@ -235,21 +276,21 @@ struct DrainParams {
   u32 n_local, stride, R, world, rank, win_cap, stamp, n_tiles;
   const u32* kinds_prev;      // [4] the kind counters the tick kernel of this tick based its dense/sparse decision on
   u64* win_data;              // my window of this exchange parity: [world][win_cap]; entries are cleared as they are consumed
-  const u32* ctrl;            // my control block of this parity: counts[8] | flags[8], written by the peers
+  const u32* counts; const u32* flags;   // my control block of this parity (ctrl_counts, ctrl_flags), written by the peers
   u32* inbox_wr;
   u8* hot_wr;
   u32* kinds_cur;             // [4] kind counters of this tick (received kinds are added so the next tick reads their planes)
   u32* overflow;
   // byzantine triples (see ByzParams): judged here against the receiver's end-of-tick record
-  u32 byz_on, byz_delta, shard_size;
+  u32 byz_on, byz_delta, shard_size, shard_inv;
   const uint4* rec; const u64* node_state;
   u8* const* peer_anomaly;    // [world] every rank's sender-flag array
   // user-event entries (KIND_EXTRA: slot = tracked event, value = its Lamport time + 1); null / 0 when user events are off
   u32 ue_n;
   u32* ue_inbox_wr;
   u32* ue_ltime;
-  // device-side sum of the tick's trace row over all ranks: grow[i] = my_row[i] + Σ peers' published rows
-  const u64* my_row; const u64* sums; u64* grow;
+  // device-side sum of the tick's trace row over all ranks: grow[i] = my_row[i] + Σ peers' published rows (ctrl_sums)
+  const u64* my_row; const CtrlRow* sums; u64* grow;
   const u32* gate;
   u32* sched_rw;              // the same words, writable: the peers' views with business are added to SCHED_VIEWS_CUR
   const u32* sched; u32* host_idle_until;   // the ranks' verdicts combined: every rank hands the same "sleep until" tick to its host
@@ -297,9 +338,7 @@ struct UeParams {
   u32* sched;                 // scheduler words of the membership kernel (idle-tick skipping): this kernel reports its activity there
   Gate gate;                  // the user-event kernel is the first kernel of a tick when user events are on
   // sharded runs: a target outside [first, first + n_local) gets one window entry per event (KIND_EXTRA) over NVLink
-  u32 world, rank, shard_size, win_cap;
-  u64* const* win_data;       // [world] peers' receive windows of this exchange parity
-  u32* send_count;            // [world] entries written into each peer's window this tick (shared with the tick kernel)
+  Sender snd;
 };
 void launch_uevent(const UeParams& p, bool trace, cudaStream_t st);
 void launch_ue_init(uint4* state, u32 n_local, cudaStream_t st);
@@ -321,13 +360,11 @@ struct ByzParams {
   // sharded runs: a peer in another shard gets a TRIPLE of window entries — serf entry and memberlist entry, both with
   // BYZ_FLAG set in the destination field, then an annotation (KIND_EXTRA, slot 15) carrying the sender's global id + 1 —
   // and the receiving shard's drain kernel judges it against ITS record and raises the flag in the sender's shard.
-  u32 n_local, world, rank, shard_size, win_cap;
-  u64* const* win_data;
-  u32* send_count;
+  u32 n_local;
+  Sender snd;
   u32* overflow;
   const u32* gate;
 };
-constexpr u32 BYZ_FLAG = 1u << 25;          // in the 26-bit destination field of a window entry (shards hold < 2^25 nodes when injectors are on)
 constexpr u32 BYZ_ANNOT_SLOT = 15;
 void launch_byz(const ByzParams& p, cudaStream_t st);
 

@@ -67,13 +67,13 @@ __global__ void __launch_bounds__(UE_BLOCK) uevent_kernel(const __grid_constant_
         if (!bits[k]) continue;
         c.edges++;
         const u32 dl = tg[k] - p.first;
-        if (p.world == 1 || dl < p.n_local) { atomicOr(p.inbox_wr + dl, bits[k]); continue; }
+        if (p.snd.world == 1 || dl < p.n_local) { atomicOr(p.inbox_wr + dl, bits[k]); continue; }
         // another shard owns the target: one 8-byte entry per event into its window (slot = event, value = ltime + 1)
-        const u32 shard = tg[k] / p.shard_size, dloc = tg[k] - shard * p.shard_size;
+        const ShardIdx t = shard_of(tg[k], p.snd.shard_size, p.snd.shard_inv);
         for (u32 e = 0; e < p.table.n; ++e) {
           if (!((bits[k] >> e) & 1u)) continue;
           const u32 Le = (stamped && e == op_slot) ? L : p.ltime[e];
-          win_append<1>(p, shard, {win_entry(Le + 1u, e, KIND_EXTRA, dloc)});
+          win_append<1>(p.snd, p.overflow, t.shard, {win_entry(Le + 1u, e, KIND_EXTRA, t.local)});
           wrote_remote = true;
         }
       }

@@ -19,6 +19,12 @@ def test_sharded_multi_slot_fanout4(world):
     P.run_against_oracle(emu_sim, scenarios.random_graph_leave(2500, 12, 4, seed=3, slots=3), world=world)
 
 
+# One node per shard: the reciprocal that maps a target to its shard has no exact u32 value for shard_size 1
+@pytest.mark.parametrize("n,world", [(3, 3), (4, 4), (8, 8)])
+def test_sharded_one_node_per_shard(n, world):
+    P.run_against_oracle(emu_sim, scenarios.full_mesh_leave(n, 3, 1), world=world)
+
+
 def test_sharded_failure_detection():
     P.run_against_oracle(emu_sim, scenarios.random_graph_fail(2000, 16, 3, seed=2), world=2, suspicion_mult=2, suspicion_max_timeout_mult=2, probe_interval_ticks=2)
 
