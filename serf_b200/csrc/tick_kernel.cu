@@ -15,8 +15,8 @@
 //
 // Memory behaviour (HBM-bound integer work, no tensor cores): one thread per node; a node's 32-byte record is one DRAM
 // sector, read as two back-to-back 128-bit loads (a warp covers 1 KB contiguous) and, if changed, written as two; node
-// word, busy byte, inbox words and row offsets are coalesced streams with an evict_first / no-L1-allocate policy; the
-// four neighbour gathers stay inside the node's own 64-byte CSR row; the sends are 32-bit RED.MAX to random peers with
+// word, queue word, busy byte and inbox words are coalesced streams with an evict_first / no-L1-allocate policy; the row
+// offsets and the four neighbour gathers (evict_first, allocated in L1) stay inside the node's own 64-byte CSR row; the sends are 32-bit RED.MAX to random peers with
 // an evict_last policy — the inbox planes are the only randomly addressed data and are sized to stay L2-resident.
 // Tiles (256 nodes) nobody delivered to and that hold no pending work are skipped outright in sparse ticks.
 // A TMA variant (tick_kernel_tma) stages whole tiles through cp.async.bulk + mbarrier; the multi-GPU variant stages
@@ -88,6 +88,20 @@ __device__ __forceinline__ void red_max_resident(u32* ptr, u32 v, u64 pol) {   /
 __device__ __forceinline__ u32 peek_inbox(const u32* ptr, u64 pol) {   // a word of the plane being reduced into (any value it held during the launch)
   u32 v; asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(ptr), "l"(pol)); return v;
 }
+__device__ __forceinline__ u32 ld_u8_stream(const u8* ptr, u64 pol) {
+  u32 v; asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(ptr), "l"(pol)); return v;
+}
+__device__ __forceinline__ u32 ld_u16_stream(const u16* ptr, u64 pol) {
+  u16 v; asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u16 %0, [%1], %2;" : "=h"(v) : "l"(ptr), "l"(pol)); return v;
+}
+__device__ __forceinline__ void st_u8_stream(u8* ptr, u32 v, u64 pol) {
+  asm volatile("st.global.L2::cache_hint.u8 [%0], %1, %2;" :: "l"(ptr), "r"(v), "l"(pol) : "memory");
+}
+// A gather from the read-only topology (no write to it during a launch: not volatile, the compiler may schedule it freely), allocated
+// in L1: the picks of a node fall into its two CSR sectors, its two row offsets into one, and the later ones hit L1.
+__device__ __forceinline__ u32 ld_topo(const u32* ptr, u64 pol) {
+  u32 v; asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(ptr), "l"(pol)); return v;
+}
 __device__ __forceinline__ void st_release_sys(u32* ptr, u32 v) { asm volatile("st.release.sys.global.u32 [%0], %1;" :: "l"(ptr), "r"(v) : "memory"); }
 __device__ __forceinline__ u32 ld_acquire_sys(const u32* ptr) { u32 f; asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(f) : "l"(ptr) : "memory"); return f; }
 #else   // SERFSIM_EMU: the same accessors as plain C++ (tests/emu compiles this file for the host; cache hints have no meaning there)
@@ -111,6 +125,35 @@ inline u32 ld_acquire_sys(const u32* ptr) {                 // polled in a loop 
   if (++spins > 64) emu::polite_wait(spins);
   return __atomic_load_n(ptr, __ATOMIC_ACQUIRE);
 }
+#endif
+
+// ---- the other per-node planes of a tick, one accessor each with its L2 policy.  Saturated ticks stream them, sparse ticks touch
+// them at a few nodes: either way nothing reads them again in the launch, and evict_first keeps them from pushing the inbox planes
+// the sends reduce into out of L2 (tools/ubench/pass_mix.cu, DESIGN §5).  Atomics on them (node_due's RED.MIN) keep the default. ----
+#ifndef SERFSIM_EMU
+__device__ __forceinline__ u32 gather_col(const u32* ptr, u64 pol) { return ld_topo(ptr, pol); }          // CSR neighbour ids
+__device__ __forceinline__ u32 ld_row_ptr(const u32* ptr, u64 pol) { return ld_topo(ptr, pol); }          // CSR row offsets (non-uniform degree)
+__device__ __forceinline__ u32 ld_qword(const u32* ptr, u64 pol) { return ld_u32_stream(ptr, pol); }      // queue words
+__device__ __forceinline__ void st_qword(u32* ptr, u32 v, u64 pol) { st_u32_stream(ptr, v, pol); }
+__device__ __forceinline__ u32 ld_busy(const u8* ptr, u64 pol) { return ld_u8_stream(ptr, pol); }        // busy bytes
+__device__ __forceinline__ void st_busy(u8* ptr, u32 v, u64 pol) { st_u8_stream(ptr, v, pol); }
+__device__ __forceinline__ u32 ld_carry(const u32* ptr, u64 pol) { return ld_u32_stream(ptr, pol); }      // carry words of the passes
+__device__ __forceinline__ void st_carry(u32* ptr, u32 v, u64 pol) { st_u32_stream(ptr, v, pol); }
+__device__ __forceinline__ u32 ld_node_due(const u32* ptr, u64 pol) { return ld_u32_stream(ptr, pol); }   // a node's own earliest deadline
+__device__ __forceinline__ void st_node_due(u32* ptr, u32 v, u64 pol) { st_u32_stream(ptr, v, pol); }
+__device__ __forceinline__ u32 ld_watch(const u16* ptr, u64 pol) { return ld_u16_stream(ptr, pol); }     // watcher masks
+#else
+inline u32 gather_col(const u32* ptr, u64) { return *ptr; }
+inline u32 ld_row_ptr(const u32* ptr, u64) { return *ptr; }
+inline u32 ld_qword(const u32* ptr, u64) { return *ptr; }
+inline void st_qword(u32* ptr, u32 v, u64) { *ptr = v; }
+inline u32 ld_busy(const u8* ptr, u64) { return *ptr; }
+inline void st_busy(u8* ptr, u32 v, u64) { *ptr = (u8)v; }
+inline u32 ld_carry(const u32* ptr, u64) { return *ptr; }
+inline void st_carry(u32* ptr, u32 v, u64) { *ptr = v; }
+inline u32 ld_node_due(const u32* ptr, u64) { return *ptr; }
+inline void st_node_due(u32* ptr, u32 v, u64) { *ptr = v; }
+inline u32 ld_watch(const u16* ptr, u64) { return *ptr; }
 #endif
 
 #ifndef SERFSIM_EMU
@@ -282,11 +325,10 @@ __device__ __forceinline__ bool flush_xwarp(const TickParams& p, XStage* xs, boo
 }
 
 // The gossip peer draw (record.cuh peer_issue) with the neighbour ids requested from the tile's stage or global memory.
-#define SFS_LD_COL(ptr, pol) __ldg(ptr)     // read-only path WITH L1 allocation: the four picks of a node fall into its two CSR sectors, later picks hit L1 (an evict_first / no-allocate gather was 6 % slower in plateau ticks)
 template <int FMAX, bool STAGED>
 __device__ __forceinline__ void pick_issue(const TickParams& p, const StageView& sv, u32 v, u32 row0, u32 deg, u64 pol_first, u32 (&cand)[FMAX]) {
   peer_issue<FMAX>(p.tick, v, p.fanout, p.seed_lo, p.seed_hi, row0, deg,
-                   [&](u32 e) { return (STAGED && sv.col_staged) ? sv.col[e - sv.col_base] : SFS_LD_COL(p.col + e, pol_first); }, cand);
+                   [&](u32 e) { return (STAGED && sv.col_staged) ? sv.col[e - sv.col_base] : gather_col(p.col + e, pol_first); }, cand);
 }
 
 // What decides whether a node has anything to do this tick: its busy byte and the inbox words of the previous tick
@@ -296,8 +338,8 @@ __device__ __forceinline__ void pick_issue(const TickParams& p, const StageView&
 // nd: the node's own earliest suspicion deadline (node_due), read only in tiles that have come due
 struct Pre { u32 busy, mL, mJ, mM, any, qw, mailmask, qmask, keep, nd; };   // mL, mJ, mM, qw: the words of view `keep` (0 in single-slot runs)
 // Carry word of node vl in this tick (CARRY_*), 0 when no earlier pass of the tick visited it.
-__device__ __forceinline__ u32 carry_of(const TickParams& p, u32 vl) {
-  const u32 w = p.carry[vl];
+__device__ __forceinline__ u32 carry_of(const TickParams& p, u32 vl, u64 pol_first) {
+  const u32 w = ld_carry(p.carry + vl, pol_first);
   return (w >> 8) == ((p.tick + 1u) & (CARRY_TICKS - 1u)) ? (w & 0xffu) : 0u;
 }
 template <bool R1, bool PASS = false>
@@ -306,15 +348,15 @@ __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool k
   // parameter block points at the active view — the distance between the planes of two kinds is p.R views either way)
   const u32 nl = p.stride, R = p.R, s_hi = R1 ? 1u : R;
   Pre x;
-  x.busy = p.busy[vl];
-  x.nd = (!R1 && due) ? p.node_due[vl] : NO_DEADLINE;    // single-view kernels (tight register cap) read it where it is needed instead: one register less across the tile loop
+  x.busy = ld_busy(p.busy + vl, pol_first);
+  x.nd = (!R1 && due) ? ld_node_due(p.node_due + vl, pol_first) : NO_DEADLINE;    // single-view kernels (tight register cap) read it where it is needed instead: one register less across the tile loop
   x.keep = R1 ? 0u : keep;
   x.mL = x.mJ = x.mM = x.qw = 0; x.any = 0; x.mailmask = 0; x.qmask = 0;
   for (u32 s2 = 0; s2 < s_hi; ++s2) {
     const u32 l = kL ? ld_u32_stream(p.inbox_rd + (size_t)(KIND_LEAVE * R + s2) * nl + vl, pol_first) : 0u;
     const u32 j = kJ ? ld_u32_stream(p.inbox_rd + (size_t)(KIND_JOIN * R + s2) * nl + vl, pol_first) : 0u;
     const u32 m = kM ? ld_u32_stream(p.inbox_rd + (size_t)(KIND_ML * R + s2) * nl + vl, pol_first) : 0u;
-    const u32 q = p.qword[(size_t)s2 * nl + vl];        // queue word (transmit budgets)
+    const u32 q = ld_qword(p.qword + (size_t)s2 * nl + vl, pol_first);        // queue word (transmit budgets)
     SFS_COUNT(6, 4);
     if (R1 || s2 == x.keep) { x.mL = l; x.mJ = j; x.mM = m; x.qw = q; }
     x.any |= l | j | m;
@@ -323,7 +365,7 @@ __device__ __forceinline__ Pre prefetch_node(const TickParams& p, u32 vl, bool k
   }
   // A pass cannot trust busy bits 0 and 3 (an earlier pass of the tick rewrote them): a queued transmit is business of the view itself,
   // and a node whose timers were due when the tick began visits every view (`any` stands for both in the activity test).
-  if (PASS) x.any |= x.qw | ((due && (carry_of(p, vl) & CARRY_TDUE)) ? 1u : 0u);
+  if (PASS) x.any |= x.qw | ((due && (carry_of(p, vl, pol_first) & CARRY_TDUE)) ? 1u : 0u);
   return x;
 }
 // Has the node anything to do this tick?  (due: its tile's earliest suspicion deadline has been reached — then a node that runs timers
@@ -450,7 +492,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
     ns = STAGED ? sv.node[lt] : ld_u64_stream(p.node_state + vl, pol_first);
     if (STAGED) { row0 = sv.rowptr[lt]; row1 = sv.rowptr[lt + 1]; }
     else if (p.udeg) { row0 = vl * p.udeg; row1 = row0 + p.udeg; }     // uniform out-degree: the row offsets are arithmetic
-    else { row0 = __ldg(p.row_ptr + vl); row1 = __ldg(p.row_ptr + vl + 1); }
+    else { row0 = ld_row_ptr(p.row_ptr + vl, pol_first); row1 = ld_row_ptr(p.row_ptr + vl + 1, pol_first); }
   };
   auto load_rec0 = [&]() {
     if (STAGED) {
@@ -468,16 +510,16 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
 
   // ---- idle exit: nothing received (any slot), nothing queued, no host operation, no probe duty, no timer due ----
   u32 nd = pre.nd;                                       // the node's own earliest deadline: matters in due tiles, for nodes that run timers
-  if (R1 && due && (busy & BUSY_TIMER)) nd = p.node_due[vl];
+  if (R1 && due && (busy & BUSY_TIMER)) nd = ld_node_due(p.node_due + vl, pol_first);
   const u32 sleeping = (due && (busy & BUSY_TIMER)) ? nd : NO_DEADLINE;
   bool timers_due = sleeping <= p.tick;
   u32 cr = 0;                                            // PASS: what the earlier passes of this tick did at this node
-  if (PASS && due) { cr = carry_of(p, vl); if (cr & CARRY_SEEN) timers_due = (cr & CARRY_TDUE) != 0; }   // as it was when the tick began
+  if (PASS && due) { cr = carry_of(p, vl, pol_first); if (cr & CARRY_SEEN) timers_due = (cr & CARRY_TDUE) != 0; }   // as it was when the tick began
   if (!TRACE && !STAGED && !(busy_business<PASS>(busy) != 0 || pre.any != 0 || p.reap_now != 0 || timers_due)) { mind = min(mind, sleeping); if (due && (busy & BUSY_TIMER)) SFS_PROBE(20); return false; }
-  if (PASS && !due) cr = carry_of(p, vl);
+  if (PASS && !due) cr = carry_of(p, vl, pol_first);
   if (STAGED && !TRACE && !(busy_business(busy) || (mL | mJ | mM) || p.reap_now || timers_due)) { mind = min(mind, sleeping); return false; }
   // (the watcher mask — subjects this node can probe, it has them as neighbours — is re-read where a watcher needs it: a handful of nodes)
-#define SFS_WMASK() ((busy & BUSY_WATCH) ? ((u32)p.watch[vl] >> p.sv_wshift) : 0u)   /* sv_wshift: the view a single-view launch works on (0 in every other launch) */
+#define SFS_WMASK() ((busy & BUSY_WATCH) ? (ld_watch(p.watch + vl, pol_first) >> p.sv_wshift) : 0u)   /* sv_wshift: the view a single-view launch works on (0 in every other launch) */
   const bool ahead = !R1 && !STAGED && ah.valid;       // node word, peers' ids and the record of view pre.keep were requested a tile ago
   if (ahead) { ns = ah.ns; row0 = vl * p.udeg; row1 = row0 + p.udeg; }
   else if (!upfront) { load_node(); if (R1) load_rec0(); }
@@ -524,7 +566,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
     const size_t idn = (size_t)s2 * nl + vl;
     w = ld_rec256(p.rec + 2 * idn, pol_first);
     if (s2 == pre.keep) { q = pre.qw; iL = pre.mL; iJ = pre.mJ; iM = pre.mM; return; }
-    q = p.qword[idn];
+    q = ld_qword(p.qword + idn, pol_first);
     SFS_COUNT(6, 4);
     iL = kL ? ld_u32_stream(p.inbox_rd + (size_t)(KIND_LEAVE * R + s2) * nl + vl, pol_first) : 0;
     iJ = kJ ? ld_u32_stream(p.inbox_rd + (size_t)(KIND_JOIN * R + s2) * nl + vl, pol_first) : 0;
@@ -638,7 +680,7 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
       Words o2 = orig, c2 = cur;                           // storage image: record without budgets, budgets in the queue word
       const u32 q_old = split_queue_word(o2), q_new = split_queue_word(c2);
       if (differs(c2, o2)) st_rec256(p.rec + 2 * idx, c2, pol_first);
-      if (q_new != q_old) { p.qword[idx] = q_new; SFS_COUNT(7, 4); }
+      if (q_new != q_old) { st_qword(p.qword + idx, q_new, pol_first); SFS_COUNT(7, 4); }
     }
     if (TRACE) c.hash += rec_hash((u64)s * p.n_global + v, cur);
     if (r.inc >= INC_LIMIT) *p.overflow = 1;
@@ -662,17 +704,17 @@ __device__ __forceinline__ bool process_node(const TickParams& p, const StageVie
   // busy byte: the op bit is consumed, the watcher bit is static; the timer bit is exact after a visit of every view and
   // sticky otherwise (a view that was not visited may run a timer: it is found when its tile comes due)
   const u32 busy2 = (awake_node ? BUSY_AWAKE : 0u) | (busy & BUSY_WATCH) | ((has_timer || (!exact && (busy & BUSY_TIMER))) ? BUSY_TIMER : 0u);
-  if (busy2 != busy) p.busy[vl] = (u8)busy2;
+  if (busy2 != busy) st_busy(p.busy + vl, busy2, pol_first);
   // node_due: a lower bound of the node's earliest running deadline, exact after a visit of every view.  A view's deadline only moves
   // while the view is visited, so views that were not visited are still covered by the word as it stands (in a pass: unless an earlier
   // pass rewrote the word exactly).
   if (has_timer) {
-    if (exact || !(busy & BUSY_TIMER)) p.node_due[vl] = mind;
+    if (exact || !(busy & BUSY_TIMER)) st_node_due(p.node_due + vl, mind, pol_first);
     else if (dl_moved || (PASS && (cr & CARRY_TDUE))) atomicMin(p.node_due + vl, mind);
   }
   if (PASS ? !timers_due : !visit_all) mind = min(mind, sleeping);   // its tile's entry was reset: timers of the views not visited go back with the node's word
   if (PASS && carry_out)                                 // a later pass of this tick has business
-    p.carry[vl] = (((p.tick + 1u) & (CARRY_TICKS - 1u)) << 8) | CARRY_SEEN | (timers_due ? CARRY_TDUE : 0u) | (awake_node ? CARRY_AWAKE : 0u) | max(pk, pk_before);
+    st_carry(p.carry + vl, (((p.tick + 1u) & (CARRY_TICKS - 1u)) << 8) | CARRY_SEEN | (timers_due ? CARRY_TDUE : 0u) | (awake_node ? CARRY_AWAKE : 0u) | max(pk, pk_before), pol_first);
   // The scheduler must know whether anybody stays awake.  A node that sent a packet this tick shows in the row's message count;
   // the others (a watcher on probe duty, a queue that has no peer to go to, a transmit queued after the send phase) are rare.
   // (a pass counts the node when its own view leaves it awake without a packet: more often than the view loop would only if a packet was
@@ -939,7 +981,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
       for (u32 g = 0; g < GROUP; ++g) {
         const bool due_g = g < ng && (hot_s[gt_s[g]] & 2u) != 0;
         Pre prg = pr[g];
-        if (due_g && (prg.busy & BUSY_TIMER)) prg.nd = p.node_due[((tile0 + gt_s[g]) << TILE_SHIFT) + threadIdx.x];
+        if (due_g && (prg.busy & BUSY_TIMER)) prg.nd = ld_node_due(p.node_due + ((tile0 + gt_s[g]) << TILE_SHIFT) + threadIdx.x, pol_first);
         const bool act = g < ng && node_active<PASS>(p, prg, due_g);   // lanes past n_local hold an empty Pre
         if (due_g) {                                         // (warp-uniform) nodes whose own timers run later hand their deadline back to the wheel
           const u32 wm = warp_min(act ? NO_DEADLINE : sleeping_deadline(prg, true));
@@ -969,7 +1011,7 @@ __global__ void __launch_bounds__(BLOCK, MB) tick_kernel(const __grid_constant__
           if (R1) {
             pre.busy = (a.x >> 16) & 0xffu; pre.any = (a.x >> 24) & 1u; pre.mL = a.y; pre.mJ = a.z; pre.mM = a.w; pre.keep = 0;
             pre.nd = NO_DEADLINE;
-            pre.qw = p.qword[vl];                             // not carried through the list: issued here, in flight with the state loads
+            pre.qw = ld_qword(p.qword + vl, pol_first);           // not carried through the list: issued here, in flight with the state loads
             pre.mailmask = pre.any ? 1u : 0u; pre.qmask = pre.qw ? 1u : 0u;
             SFS_COUNT(6, 4);
           } else {
